@@ -330,6 +330,10 @@ int loam_b200_map_surround_async(loam_b200_ctx* ctx, const int cen[3], const int
  * (BasicLaserMapping.cpp:503-509: the map points of the cubes in view) in the *_FROM_MAP cloud slots.  Off by default:
  * the persistent cell-sorted map never needs that copy, only its size (sizes_out[0..1]). */
 int loam_b200_map_debug_from_map(loam_b200_ctx* ctx, int on);
+/* Test switch: cell pruning of the scan-to-map search over the persistent map (cells a query cannot reach within 1 m are
+ * not probed).  mode -1 (default): on when the map's points take more than half of the device's L2; 0 off; 1 on.  The
+ * search result does not depend on it. */
+int loam_b200_debug_map_prune(loam_b200_ctx* ctx, int mode);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice

@@ -71,6 +71,9 @@ class MapWindow(C.Structure):
 
 
 TREE_ODOM_CORNER, TREE_ODOM_SURF, TREE_MAP_CORNER, TREE_MAP_SURF = range(4)
+# cloud slots of the mapping stage (include/loam_b200.h)
+(C_MAP_CORNER_LAST, C_MAP_SURF_LAST, C_MAP_FULL, C_MAP_CORNER_STACK_DS, C_MAP_SURF_STACK_DS, C_MAP_CORNER_FROM_MAP,
+ C_MAP_SURF_FROM_MAP, C_MAP_SURROUND_DS, C_MAP_CORNER_POOL, C_MAP_SURF_POOL) = range(12, 22)
 K_FEATURES, K_TREE_BUILD, K_KNN, K_MAP_ITER, K_ODOM_ITER, K_TRANSFORM, K_VOXEL = range(7)
 KERNEL_FAMILIES = ["features", "tree_build", "knn", "map_iter", "odom_iter", "transform", "voxel"]
 
@@ -142,6 +145,7 @@ def lib():
         "loam_b200_map_surround": (C.c_int, [vp, _I, _I, C.c_int, C.c_float]),
         "loam_b200_map_surround_async": (C.c_int, [vp, _I, _I, C.c_int, C.c_float]),
         "loam_b200_map_debug_from_map": (C.c_int, [vp, C.c_int]),
+        "loam_b200_debug_map_prune": (C.c_int, [vp, C.c_int]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -236,14 +240,30 @@ def _pts(a):
     return a.reshape(-1, 4)
 
 
+_libm = None
+
+
+def sincos_f32(angle):
+    """(sinf(angle), cosf(angle)) from the C math library, as loam::Angle caches them (std::sin / std::cos of a float).
+    numpy's float32 sin / cos round differently for a good share of angles beyond a few tenths of a radian."""
+    global _libm
+    if _libm is None:
+        import ctypes.util
+        _libm = C.CDLL(ctypes.util.find_library("m") or "libm.so.6")
+        for fn in (_libm.sinf, _libm.cosf):
+            fn.restype = C.c_float
+            fn.argtypes = [C.c_float]
+    a = float(np.float32(angle))
+    return np.float32(_libm.sinf(a)), np.float32(_libm.cosf(a))
+
+
 def make_pose(twist6) -> Pose:
     """Pose struct from (rot_x, rot_y, rot_z, x, y, z) with float sin/cos like loam::Angle caches them."""
     t = np.asarray(twist6, dtype=np.float32)
     p = Pose()
     for i in range(3):
         p.rot[i] = t[i]
-        p.sin_[i] = np.sin(t[i], dtype=np.float32)
-        p.cos_[i] = np.cos(t[i], dtype=np.float32)
+        p.sin_[i], p.cos_[i] = sincos_f32(t[i])
         p.pos[i] = t[3 + i]
     return p
 
@@ -253,8 +273,7 @@ def make_odom_pose(twist6, scan_period=0.1, it=0) -> OdomPose:
     p = OdomPose()
     for i in range(3):
         p.rot[i] = t[i]
-        p.sin_[i] = np.sin(t[i], dtype=np.float32)
-        p.cos_[i] = np.cos(t[i], dtype=np.float32)
+        p.sin_[i], p.cos_[i] = sincos_f32(t[i])
         p.pos[i] = t[3 + i]
     p.inv_scan_period = np.float32(1.0) / np.float32(scan_period)
     p.iter = it
@@ -345,6 +364,53 @@ class Ctx:
         c, s = _pts(corner), _pts(surf)
         self._ck(self.L.loam_b200_map_set_queries(self.h, _fp(c), c.shape[0], _fp(s), s.shape[0]), "map_set_queries")
         self._nq = c.shape[0] + s.shape[0]
+
+    # ---- mapping stage (device-resident map; include/loam_b200.h "Mapping stage")
+    def cloud_upload(self, slot, pts):
+        a = _pts(pts)
+        self._ck(self.L.loam_b200_cloud_upload(self.h, slot, _fp(a), a.shape[0]), "cloud_upload")
+
+    def cloud_download(self, slot):
+        n = self.L.loam_b200_cloud_size(self.h, slot)
+        if n < 0:
+            self._ck(n, "cloud_size")
+        out = np.empty((max(n, 1), 4), np.float32)
+        got = C.c_int(0)
+        self._ck(self.L.loam_b200_cloud_download(self.h, slot, _fp(out), out.shape[0], C.byref(got)), "cloud_download")
+        return out[:got.value].copy()
+
+    def map_pool_append(self, kind, pts):
+        a = _pts(pts)
+        self._ck(self.L.loam_b200_map_pool_append(self.h, kind, _fp(a), a.shape[0]), "map_pool_append")
+
+    def map_begin_sweep(self, twist6, cen, valid_cubes, corner_leaf=0.2, surf_leaf=0.4):
+        """Window + stacks of one sweep -> sizes_out[4] (from-map corner / surface counts, corner / surface stack sizes);
+        map_iterate then runs over the persistent map with the down-sized stacks as queries."""
+        p = make_pose(twist6)
+        cubes = np.ascontiguousarray(valid_cubes, dtype=np.int32).reshape(-1)
+        win = MapWindow()
+        for i in range(3):
+            win.cen[i] = int(cen[i])
+        win.valid_cubes = _ip(cubes) if cubes.size else None
+        win.n_valid = cubes.size
+        win.corner_leaf = corner_leaf
+        win.surf_leaf = surf_leaf
+        sizes = np.zeros(4, np.int32)
+        self._ck(self.L.loam_b200_map_begin_sweep(self.h, C.byref(p), C.byref(win), _ip(sizes)), "map_begin_sweep")
+        self._nq = int(sizes[2]) + int(sizes[3])
+        return sizes
+
+    def map_end_sweep(self, twist6, asynchronous=False):
+        p = make_pose(twist6)
+        fn = self.L.loam_b200_map_end_sweep_async if asynchronous else self.L.loam_b200_map_end_sweep
+        self._ck(fn(self.h, C.byref(p)), "map_end_sweep")
+
+    def map_debug_from_map(self, on=True):
+        self._ck(self.L.loam_b200_map_debug_from_map(self.h, 1 if on else 0), "map_debug_from_map")
+
+    def debug_map_prune(self, mode):
+        """-1 automatic (from the L2 size), 0 off, 1 on."""
+        self._ck(self.L.loam_b200_debug_map_prune(self.h, mode), "debug_map_prune")
 
     def map_iterate(self, twist6, debug=False):
         p = make_pose(twist6)

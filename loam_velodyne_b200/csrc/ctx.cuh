@@ -321,6 +321,7 @@ struct loam_b200_ctx {
   } store[2];
   bool map_use_store = false;      // scan-to-map search goes through the store (stage API) / through grid[] (kernel API)
   bool map_debug_from_map = false; // begin_sweep also materialises the from-map clouds (tests)
+  int map_prune_mode = -1;          // cell pruning of the store search: -1 from the L2 size, 0 off, 1 on (tests)
   loamb::DevBuf<float4> pool_tmp;
   loamb::DevBuf<unsigned char> pool_tmp_cls;
   loamb::DevBuf<unsigned> cmp_pos, cmp_bsum;

@@ -139,7 +139,7 @@ MapCellLookup store_lookup_of(const loam_b200_ctx* c, int kind) {
   lk.ax = lk.ay = lk.az = CellAxis{0, 0, 0};
   // maps whose points (16 B each) take more than half of L2 are fetched from HBM: prune the unreachable cells there
   const long long map_pts = (long long)c->cloud_n[LOAM_B200_C_MAP_CORNER_POOL] + c->cloud_n[LOAM_B200_C_MAP_SURF_POOL];
-  lk.prune = map_pts * 16 > (long long)c->l2_bytes / 2 ? 1 : 0;
+  lk.prune = c->map_prune_mode >= 0 ? c->map_prune_mode : (map_pts * 16 > (long long)c->l2_bytes / 2 ? 1 : 0);
   return lk;
 }
 
@@ -644,6 +644,11 @@ int loam_b200_create(loam_b200_ctx** out, int device) {
     return LOAM_B200_ERR_CUDA;
   }
   cudaMemsetAsync(c->ticket.p, 0, 4 * sizeof(unsigned), c->stream);
+  // Pinned memory comes back from the allocator as its previous owner left it, e.g. a destroyed context's mailbox holding
+  // the sequence number this context's first post will use: the host would take that stale content for the post.  The
+  // mailboxes start from zero, which no post carries (sequence numbers run from 1).
+  memset(c->result_mailbox.p, 0, 64 * sizeof(float));
+  memset(c->int_mailbox.p, 0, 512 * sizeof(int));
   cudaStreamSynchronize(c->stream);
   *out = c;
   return LOAM_B200_OK;

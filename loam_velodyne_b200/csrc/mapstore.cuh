@@ -15,7 +15,9 @@
 // dimensions of its ABSOLUTE cube coordinates, so keys do not change when the grid rolls (:311-441 only changes the
 // centre offsets); points of cubes that left the grid are dropped by the merge of the sweep in which the roll happened.
 // A point is RAW until a voxel filter has seen it: seeded maps and points inserted into cubes outside the field of view
-// stay unfiltered, exactly like the reference's cube clouds, until their cube is visible at the end of a sweep.
+// stay unfiltered, exactly like the reference's cube clouds, until their cube is visible at the end of a sweep.  So does
+// a centroid that rounded out of its voxel (store_voxel_merge_kernel): the reference's next filter of the cube sees it
+// in the voxel it landed in.
 #pragma once
 
 #include "gridnn.cuh"
@@ -340,7 +342,11 @@ __global__ void store_voxel_merge_kernel(const float4* __restrict__ s_pts, const
   const float fn = (float)cnt;
   const float4 c = make_float4(sx / fn, sy / fn, sz / fn, si / fn);
   e_pts[dst] = c;
-  e_state[dst] = 0;
+  // An fp32 centroid can round across a voxel face (three points at x = -53.200005 average to -53.2, one 0.2 m voxel
+  // up).  The reference re-filters the whole cube whenever it is in view, which then merges that centroid with the
+  // voxel it landed in; kept RAW, the point takes part in the filter of the next sweep that sees its cube, like that.
+  const bool left_voxel = floorf(c.x * inv_leaf) != fvx || floorf(c.y * inv_leaf) != fvy || floorf(c.z * inv_leaf) != fvz;
+  e_state[dst] = left_voxel ? ST_RAW : 0;
   e_keys[dst] = torus_key_of(c);
   e_vals[dst] = (int)dst;
 }

@@ -334,6 +334,15 @@ int loam_b200_map_debug_from_map(loam_b200_ctx* ctx, int on);
  * not probed).  mode -1 (default): on when the map's points take more than half of the device's L2; 0 off; 1 on.  The
  * search result does not depend on it. */
 int loam_b200_debug_map_prune(loam_b200_ctx* ctx, int mode);
+/* Test switch: the scan-to-scan correspondence search scans a ring-ordered last cloud (ring ids 0..255 in ascending order)
+ * as two index ranges from its ring offset table.  mode 1 (default): automatic; 0: always the serial scan with the ring
+ * `break` (the path every other cloud takes).  Reaches loam_b200_odom_iterate* and loam_b200_odom_solve; the search result
+ * does not depend on it. */
+int loam_b200_debug_odom_ring_ranges(loam_b200_ctx* ctx, int mode);
+/* Test query: how the last build of tree `slot` ran (joins a pending loam_b200_odom_rebuild_last first). */
+enum { LOAM_B200_BUILD_NONE = 0, LOAM_B200_BUILD_CLUSTER_PAIR = 1, LOAM_B200_BUILD_CLUSTER = 2,
+       LOAM_B200_BUILD_MULTI_LAUNCH = 3 };
+int loam_b200_debug_tree_build_path(loam_b200_ctx* ctx, int slot);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice

@@ -71,6 +71,10 @@ class MapWindow(C.Structure):
 
 
 TREE_ODOM_CORNER, TREE_ODOM_SURF, TREE_MAP_CORNER, TREE_MAP_SURF = range(4)
+BUILD_NONE, BUILD_CLUSTER_PAIR, BUILD_CLUSTER, BUILD_MULTI_LAUNCH = range(4)
+# cloud slots of the registration and odometry stages (include/loam_b200.h)
+(C_REG_FULL, C_REG_SHARP, C_REG_LESS_SHARP, C_REG_FLAT, C_REG_LESS_FLAT, C_ODOM_SHARP, C_ODOM_LESS_SHARP, C_ODOM_FLAT,
+ C_ODOM_LESS_FLAT, C_ODOM_FULL, C_ODOM_LAST_CORNER, C_ODOM_LAST_SURF) = range(12)
 # cloud slots of the mapping stage (include/loam_b200.h)
 (C_MAP_CORNER_LAST, C_MAP_SURF_LAST, C_MAP_FULL, C_MAP_CORNER_STACK_DS, C_MAP_SURF_STACK_DS, C_MAP_CORNER_FROM_MAP,
  C_MAP_SURF_FROM_MAP, C_MAP_SURROUND_DS, C_MAP_CORNER_POOL, C_MAP_SURF_POOL) = range(12, 22)
@@ -146,6 +150,8 @@ def lib():
         "loam_b200_map_surround_async": (C.c_int, [vp, _I, _I, C.c_int, C.c_float]),
         "loam_b200_map_debug_from_map": (C.c_int, [vp, C.c_int]),
         "loam_b200_debug_map_prune": (C.c_int, [vp, C.c_int]),
+        "loam_b200_debug_odom_ring_ranges": (C.c_int, [vp, C.c_int]),
+        "loam_b200_debug_tree_build_path": (C.c_int, [vp, C.c_int]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -379,6 +385,9 @@ class Ctx:
         self._ck(self.L.loam_b200_cloud_download(self.h, slot, _fp(out), out.shape[0], C.byref(got)), "cloud_download")
         return out[:got.value].copy()
 
+    def cloud_swap(self, a, b):
+        self._ck(self.L.loam_b200_cloud_swap(self.h, a, b), "cloud_swap")
+
     def map_pool_append(self, kind, pts):
         a = _pts(pts)
         self._ck(self.L.loam_b200_map_pool_append(self.h, kind, _fp(a), a.shape[0]), "map_pool_append")
@@ -411,6 +420,36 @@ class Ctx:
     def debug_map_prune(self, mode):
         """-1 automatic (from the L2 size), 0 off, 1 on."""
         self._ck(self.L.loam_b200_debug_map_prune(self.h, mode), "debug_map_prune")
+
+    # ---- odometry stage (include/loam_b200.h "Odometry stage"): last clouds and queries from the cloud slots
+    def odom_adopt(self, src: "Ctx", src5):
+        """The registration -> odometry hand-off from `src`'s slots src5 (sharp, less sharp, flat, less flat, full)."""
+        s = np.ascontiguousarray(src5, dtype=np.int32).reshape(5)
+        self._ck(self.L.loam_b200_odom_adopt(self.h, src.h, _ip(s)), "odom_adopt")
+
+    def odom_prepare(self):
+        """This sweep's queries from the ODOM_SHARP / ODOM_FLAT slots; odom_iterate / odom_solve then search them."""
+        self._ck(self.L.loam_b200_odom_prepare(self.h), "odom_prepare")
+        self._noq = (self.L.loam_b200_cloud_size(self.h, C_ODOM_SHARP) + self.L.loam_b200_cloud_size(self.h, C_ODOM_FLAT))
+
+    def odom_rebuild_last(self):
+        """Trees and ring offsets of the ODOM_LAST_CORNER / ODOM_LAST_SURF slots (built asynchronously)."""
+        self._ck(self.L.loam_b200_odom_rebuild_last(self.h), "odom_rebuild_last")
+
+    def cloud_transform_to_end2(self, slot_a, slot_b, twist6, scan_period=0.1):
+        p = make_odom_pose(twist6, scan_period, 0)
+        self._ck(self.L.loam_b200_cloud_transform_to_end2(self.h, slot_a, slot_b, C.byref(p)), "cloud_transform_to_end2")
+
+    def debug_odom_ring_ranges(self, mode):
+        """1 automatic (index ranges on ring-ordered last clouds), 0 always the serial scan."""
+        self._ck(self.L.loam_b200_debug_odom_ring_ranges(self.h, mode), "debug_odom_ring_ranges")
+
+    def debug_tree_build_path(self, slot):
+        """BUILD_CLUSTER_PAIR, BUILD_CLUSTER or BUILD_MULTI_LAUNCH: how tree `slot` was last built."""
+        rc = self.L.loam_b200_debug_tree_build_path(self.h, slot)
+        if rc < 0:
+            self._ck(rc, "debug_tree_build_path")
+        return rc
 
     def map_iterate(self, twist6, debug=False):
         p = make_pose(twist6)

@@ -33,7 +33,7 @@ constexpr int CS_CL = LOAM_B200_CS_CL;
 constexpr int CS_THREADS = LOAM_B200_CS_THREADS;
 constexpr int CS_NW = CS_THREADS / 32;
 constexpr int CS_CAP = 8192;              // pairs per CTA
-constexpr int CS_MAX_N = CS_CL * CS_CAP;  // 65536
+constexpr int CS_MAX_N = CS_CL * CS_CAP;  // 131072 with 16 CTAs
 
 struct ClusterSortSmem {
   unsigned keys[2][CS_CAP];

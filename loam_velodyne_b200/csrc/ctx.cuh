@@ -116,6 +116,7 @@ struct Tree {
   DevBuf<int> parent;      // parent of internal node i / of leaf (stored at n_leaf-1+leaf)
   DevBuf<int> flags;
   DevBuf<float4> box_lo, box_hi;  // per-node total boxes during refit (internal then leaves)
+  int build_path = 0;  // how the last build ran (LOAM_B200_BUILD_*, loam_b200_debug_tree_build_path)
 };
 
 struct FeatSlots { int cap_sharp = 0, cap_less = 0, cap_flat = 0; };
@@ -286,8 +287,11 @@ struct loam_b200_ctx {
   bool od_last_set = false;
   bool od_rebuild_pending = false;
   int od_rebuild_lanes = 2;    // side lanes the pending rebuild runs on
-  bool od_prepared = false;    // od_q already holds this sweep's queries (loam_b200_odom_adopt)
+  bool od_prepared = false;    // od_q already holds this sweep's queries (loam_b200_odom_adopt); any later write to
+                               // the ODOM_SHARP / ODOM_FLAT slots clears it
   loamb::DevBuf<int> od_ring_off[2];  // ring offset tables of the last corner / surface clouds (odometry_lm.cuh)
+  bool od_ring_ranges = true;  // the search may scan ring-ordered last clouds as index ranges; false: always the
+                               // serial scan (tests)
 
   // device-resident clouds of the stage API
   loamb::DevBuf<float4> cloud[LOAM_B200_NUM_CLOUDS];

@@ -185,6 +185,8 @@ int grid_build_device(loam_b200_ctx* c, Grid& g, const float4* d_pts, int m, con
 
 // ring offset tables of the odometry's last-sweep clouds (odometry_lm.cuh: ring_offsets_kernel); both live in one buffer
 int* ring_off_ptr(loam_b200_ctx* c, int kind) { return c->od_ring_off[0].p ? c->od_ring_off[0].p + kind * RING_OFF_WORDS : nullptr; }
+// ... as the search kernels get it: none makes them take the serial scan (loam_b200_debug_odom_ring_ranges)
+const int* ring_off_search(loam_b200_ctx* c, int kind) { return c->od_ring_ranges ? ring_off_ptr(c, kind) : nullptr; }
 int odom_ring_offsets(loam_b200_ctx* c, int kind, const float4* d_pts, int m) {
   LB_CUDA(c, c->od_ring_off[0].reserve(2 * RING_OFF_WORDS));
   LB_CUDA(c, cudaMemsetAsync(ring_off_ptr(c, kind), 0, RING_OFF_WORDS * sizeof(int), c->stream));
@@ -238,6 +240,7 @@ int tree_build_pair_cluster(loam_b200_ctx* c, Tree& t0, int m0, Tree& t1, int m1
   LB_LAUNCH_CHECK(c);
   t0.root = t0.n_leaf == 1 ? ~0 : 0;
   t1.root = t1.n_leaf == 1 ? ~0 : 0;
+  t0.build_path = t1.build_path = LOAM_B200_BUILD_CLUSTER_PAIR;
   *done = true;
   return LOAM_B200_OK;
 }
@@ -246,6 +249,7 @@ int tree_build_pair_cluster(loam_b200_ctx* c, Tree& t0, int m0, Tree& t1, int m1
 int tree_build_device(loam_b200_ctx* c, Tree& t, int m) {
   int rc0 = tree_reserve(c, t, m);
   if (rc0) return rc0;
+  t.build_path = LOAM_B200_BUILD_NONE;
   if (m <= 0) return LOAM_B200_OK;
   const int n_leaf = t.n_leaf;
   if (cluster_path_ok(c, m)) {
@@ -253,8 +257,10 @@ int tree_build_device(loam_b200_ctx* c, Tree& t, int m) {
     bvh_build_cluster_kernel<<<CS_CL, CS_THREADS, sizeof(ClusterSortSmem), c->stream>>>(bvh_args_of(t), none);
     LB_LAUNCH_CHECK(c);
     t.root = n_leaf == 1 ? ~0 : 0;
+    t.build_path = LOAM_B200_BUILD_CLUSTER;
     return LOAM_B200_OK;
   }
+  t.build_path = LOAM_B200_BUILD_MULTI_LAUNCH;
   SortScratch& s = c->sort;
   LB_CUDA(c, s.keys_a.reserve(m));
   LB_CUDA(c, s.keys_b.reserve(m));
@@ -1178,7 +1184,7 @@ static int odom_iterate_impl(loam_b200_ctx* c, const loam_b200_odom_pose* pose, 
     const int warps = nsh + nfl;
     odom_search_kernel<false><<<blocks_for((long long)warps * 32, LM_THREADS), LM_THREADS, 0, c->stream>>>(
         view_of(tc), view_of(ts), tc.points(), ts.points(), c->od_q.p, nsh, nfl, a, c->od_ind.p, nullptr,
-        ring_off_ptr(c, 0), ring_off_ptr(c, 1));
+        ring_off_search(c, 0), ring_off_search(c, 1));
     LB_LAUNCH_CHECK(c);
   }
   ResultMailbox mb{nullptr, 0};
@@ -1314,7 +1320,7 @@ int loam_b200_odom_solve(loam_b200_ctx* c, const float rot[3], const float pos[3
   OdomLoopIo io;
   io.corner_tree = view_of(tc); io.surf_tree = view_of(ts);
   io.last_corner = tc.points(); io.last_surf = ts.points(); io.queries = c->od_q.p; io.ind = c->od_ind.p;
-  io.ring_off_corner = ring_off_ptr(c, 0); io.ring_off_surf = ring_off_ptr(c, 1);
+  io.ring_off_corner = ring_off_search(c, 0); io.ring_off_surf = ring_off_search(c, 1);
   io.n_sharp = nsh; io.n_flat = nfl; io.sharp_blocks = cb; io.n_blocks = nb;
   odom_lm_init_kernel<<<1, 32, 0, c->stream>>>(st, rot[0], rot[1], rot[2], pos[0], pos[1], pos[2], inv_scan_period,
                                                delta_t_abort, delta_r_abort, max_iterations, tc.m, ts.m, io, seq);

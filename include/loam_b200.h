@@ -345,6 +345,34 @@ enum { LOAM_B200_BUILD_NONE = 0, LOAM_B200_BUILD_CLUSTER_PAIR = 1, LOAM_B200_BUI
 int loam_b200_debug_tree_build_path(loam_b200_ctx* ctx, int slot);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Whole-run voxel map (optional, off by default; csrc/densemap.cuh, DESIGN.md "Whole-run voxel map").  Once enabled,
+ * every loam_b200_map_end_sweep(_async) adds the registered full-resolution cloud (MAP_FULL, map frame) to a persistent
+ * device hash table of voxels that is never rolled or pruned.  Voxel of a point: (int)floorf(c * (1.0f / leaf)) per
+ * axis (PCL VoxelGrid's index before min_b); voxels beyond [-2^20, 2^20) on an axis and non-finite points are skipped.
+ * Per voxel: count and fp64 sums, added sequentially in ascending cloud index within a sweep and sweep by sweep; export
+ * gives (float)(sum / count) of x, y, z and intensity in ascending voxel order (z-major, x fastest: VoxelGrid's order).
+ * When a sweep brings more new voxels than max_voxels leaves room for, they are admitted in ascending voxel order until
+ * the table is full and the points of the others are counted as dropped.  The insertion of the mapping stage runs on a
+ * stream of its own beside the map update; the next write into MAP_FULL (loam_b200_cloud_upload / _copy / _copy_many /
+ * _swap / the in-place transforms, which the drop-in's adopt / laserCloud() / process use) waits for it.
+ *   enable: leaf finite and > 0, 1 <= max_voxels <= 2^31 - 1 (else LOAM_B200_ERR_ARG); another leaf while the map holds
+ *           voxels, or a sharded context (loam_b200_map_set_shard / comm / peer), gives LOAM_B200_ERR_STATE.  The same
+ *           leaf again changes the cap; a cap below the stored voxels keeps them (and their accumulation) and admits
+ *           no new voxel.
+ *   insert: accumulate the cloud in any slot (kernel-level use and tests; the mapping stage inserts MAP_FULL itself);
+ *           everything enqueued on the context afterwards waits for it, since stage calls write some slots directly.
+ *   stats:  out3 = voxels, skipped points, dropped points (synchronises).
+ *   export: every voxel as packed float[4] centroids (+ counts when counts != NULL); *n_out = number of voxels,
+ *           LOAM_B200_ERR_CAPACITY when it exceeds cap (synchronises).  Not enabled: an empty map.
+ *   clear:  empty the map (the leaf may then change).
+ * ------------------------------------------------------------------------------------------------------------------ */
+int loam_b200_dense_enable(loam_b200_ctx* ctx, float leaf, long long max_voxels);
+int loam_b200_dense_insert(loam_b200_ctx* ctx, int slot);
+int loam_b200_dense_stats(loam_b200_ctx* ctx, long long out3[3]);
+int loam_b200_dense_export(loam_b200_ctx* ctx, float* xyzi, uint32_t* counts, int cap, int* n_out);
+int loam_b200_dense_clear(loam_b200_ctx* ctx);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice
  * of the corner and surface queries; with a communicator the 32-float partial normal equations are all-reduced
  * (NCCL, sum, fp32) on the context's stream directly behind the kernel, so every rank returns the same totals and
@@ -361,7 +389,8 @@ int loam_b200_map_set_shard(loam_b200_ctx* ctx, int rank, int world);
  * launch counts per kernel family since the last reset.
  * ------------------------------------------------------------------------------------------------------------------ */
 enum { LOAM_B200_K_FEATURES = 0, LOAM_B200_K_TREE_BUILD = 1, LOAM_B200_K_KNN = 2, LOAM_B200_K_MAP_ITER = 3,
-       LOAM_B200_K_ODOM_ITER = 4, LOAM_B200_K_TRANSFORM = 5, LOAM_B200_K_VOXEL = 6, LOAM_B200_NUM_KERNEL_FAMILIES = 7 };
+       LOAM_B200_K_ODOM_ITER = 4, LOAM_B200_K_TRANSFORM = 5, LOAM_B200_K_VOXEL = 6, LOAM_B200_K_DENSE = 7,
+       LOAM_B200_NUM_KERNEL_FAMILIES = 8 };
 int loam_b200_profile_enable(loam_b200_ctx* ctx, int on);
 int loam_b200_profile_reset(loam_b200_ctx* ctx);
 int loam_b200_profile_get(loam_b200_ctx* ctx, int family, double* gpu_ms, long long* launches);

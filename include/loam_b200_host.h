@@ -91,6 +91,15 @@ int loam_b200_map_kernel_profile(void* h, int reps, double* out5);
 int loam_b200_map_kernel_profile_queries(void* h, const float* queries, int n, int reps, double* out5);
 /* test hook: keep a copy of laserCloudCornerFromMap / laserCloudSurfFromMap (cloud ids 2, 3) at every process() */
 int loam_b200_map_retain_from_map(void* h, int on);
+/* whole-run voxel map (BasicLaserMapping::enableDenseMap & co., include/loam_b200.h "Whole-run voxel map"):
+ * stats out3 = voxels, skipped points, dropped points; export writes n_out packed float[4] centroids (+ counts when
+ * counts != NULL) in ascending voxel order, LOAM_B200_ERR_CAPACITY (with *n_out set) when they exceed cap.  On a
+ * streaming pipeline's mapping object these four return LOAM_B200_ERR_STATE while sweeps are in flight, i.e. from
+ * loam_b200_pipeline_submit until loam_b200_pipeline_collect has returned that sweep's result. */
+int loam_b200_map_dense_enable(void* h, float leaf, long long max_voxels);
+int loam_b200_map_dense_stats(void* h, long long* out3);
+int loam_b200_map_dense_export(void* h, float* xyzi, unsigned int* counts, int cap, int* n_out);
+int loam_b200_map_dense_clear(void* h);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank
  * then enables sharding on its mapping object (nccl_id128 = NULL: slice the queries only, no collective) */
 int loam_b200_host_nccl_unique_id(unsigned char* out128);

@@ -78,8 +78,11 @@ BUILD_NONE, BUILD_CLUSTER_PAIR, BUILD_CLUSTER, BUILD_MULTI_LAUNCH = range(4)
 # cloud slots of the mapping stage (include/loam_b200.h)
 (C_MAP_CORNER_LAST, C_MAP_SURF_LAST, C_MAP_FULL, C_MAP_CORNER_STACK_DS, C_MAP_SURF_STACK_DS, C_MAP_CORNER_FROM_MAP,
  C_MAP_SURF_FROM_MAP, C_MAP_SURROUND_DS, C_MAP_CORNER_POOL, C_MAP_SURF_POOL) = range(12, 22)
-K_FEATURES, K_TREE_BUILD, K_KNN, K_MAP_ITER, K_ODOM_ITER, K_TRANSFORM, K_VOXEL = range(7)
-KERNEL_FAMILIES = ["features", "tree_build", "knn", "map_iter", "odom_iter", "transform", "voxel"]
+K_FEATURES, K_TREE_BUILD, K_KNN, K_MAP_ITER, K_ODOM_ITER, K_TRANSFORM, K_VOXEL, K_DENSE = range(8)
+KERNEL_FAMILIES = ["features", "tree_build", "knn", "map_iter", "odom_iter", "transform", "voxel", "dense"]
+_U = C.POINTER(C.c_uint32)
+_LL = C.POINTER(C.c_longlong)
+DENSE_MAX_VOXELS = 2**31 - 1  # default cap of the whole-run voxel map: none below the export's int32 count
 
 _lib = None
 
@@ -152,6 +155,11 @@ def lib():
         "loam_b200_debug_map_prune": (C.c_int, [vp, C.c_int]),
         "loam_b200_debug_odom_ring_ranges": (C.c_int, [vp, C.c_int]),
         "loam_b200_debug_tree_build_path": (C.c_int, [vp, C.c_int]),
+        "loam_b200_dense_enable": (C.c_int, [vp, C.c_float, C.c_longlong]),
+        "loam_b200_dense_insert": (C.c_int, [vp, C.c_int]),
+        "loam_b200_dense_stats": (C.c_int, [vp, _LL]),
+        "loam_b200_dense_export": (C.c_int, [vp, _F, _U, C.c_int, _I]),
+        "loam_b200_dense_clear": (C.c_int, [vp]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -196,6 +204,10 @@ def lib():
         "loam_b200_map_last_iterations": (C.c_int, [vp]),
         "loam_b200_map_last_phase_seconds": (C.c_int, [vp, _D]),
         "loam_b200_map_retain_from_map": (C.c_int, [vp, C.c_int]),
+        "loam_b200_map_dense_enable": (C.c_int, [vp, C.c_float, C.c_longlong]),
+        "loam_b200_map_dense_stats": (C.c_int, [vp, _LL]),
+        "loam_b200_map_dense_export": (C.c_int, [vp, _F, _U, C.c_int, _I]),
+        "loam_b200_map_dense_clear": (C.c_int, [vp]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_map_kernel_profile": (C.c_int, [vp, C.c_int, _D]),
@@ -545,6 +557,28 @@ class Ctx:
                                              C.byref(n)), "voxel_grid")
         return out[:n.value].copy()
 
+    # ---- whole-run voxel map (include/loam_b200.h "Whole-run voxel map")
+    def dense_enable(self, leaf, max_voxels=DENSE_MAX_VOXELS):
+        self._ck(self.L.loam_b200_dense_enable(self.h, np.float32(leaf), int(max_voxels)), "dense_enable")
+
+    def dense_insert(self, slot):
+        """Accumulate the cloud in `slot` (fill it with cloud_upload)."""
+        self._ck(self.L.loam_b200_dense_insert(self.h, slot), "dense_insert")
+
+    def dense_stats(self):
+        """{"voxels", "skipped", "dropped"} (synchronises)."""
+        out = np.zeros(3, np.int64)
+        self._ck(self.L.loam_b200_dense_stats(self.h, out.ctypes.data_as(_LL)), "dense_stats")
+        return _dense_stats(out)
+
+    def dense_export(self):
+        """(centroids N x 4 float32, counts N uint32) in ascending voxel order."""
+        return _dense_export(lambda pts, cnt, cap, n: self.L.loam_b200_dense_export(self.h, pts, cnt, cap, n),
+                             self.dense_stats()["voxels"], lambda rc: self._ck(rc, "dense_export"))
+
+    def dense_clear(self):
+        self._ck(self.L.loam_b200_dense_clear(self.h), "dense_clear")
+
     def profile(self, on=True):
         self.L.loam_b200_profile_enable(self.h, 1 if on else 0)
         self.L.loam_b200_profile_reset(self.h)
@@ -560,6 +594,18 @@ class Ctx:
 
     def launch_count(self):
         return self.L.loam_b200_launch_count(self.h)
+
+
+def _dense_stats(out):
+    return {"voxels": int(out[0]), "skipped": int(out[1]), "dropped": int(out[2])}
+
+
+def _dense_export(fn, n, ck):
+    pts = np.zeros((max(n, 1), 4), np.float32)
+    cnt = np.zeros(max(n, 1), np.uint32)
+    got = C.c_int(0)
+    ck(fn(_fp(pts), cnt.ctypes.data_as(_U), n, C.byref(got)))
+    return pts[:got.value].copy(), cnt[:got.value].copy()
 
 
 def _ne(ne: NormalEq):
@@ -713,6 +759,25 @@ class LaserMapping(_Handle):
         out = np.zeros(4, np.float64)
         self.L.loam_b200_map_last_phase_seconds(self.h, out.ctypes.data_as(_D))
         return dict(zip(["begin_sweep", "lm_loop", "end_sweep", "surround"], np.round(out * 1e3, 3)))
+
+    # ---- whole-run voxel map (BasicLaserMapping::enableDenseMap & co.)
+    def enable_dense_map(self, leaf, max_voxels=DENSE_MAX_VOXELS):
+        """Accumulate every mapped sweep's registered full-resolution cloud into a voxel map on the GPU (off by default)."""
+        self._ck(self.L.loam_b200_map_dense_enable(self.h, np.float32(leaf), int(max_voxels)), "enableDenseMap")
+
+    def dense_stats(self):
+        """{"voxels", "skipped", "dropped"} of the whole-run voxel map."""
+        out = np.zeros(3, np.int64)
+        self._ck(self.L.loam_b200_map_dense_stats(self.h, out.ctypes.data_as(_LL)), "denseMapStats")
+        return _dense_stats(out)
+
+    def dense_map(self):
+        """(centroids N x 4 float32: x, y, z, intensity; counts N uint32) in ascending voxel order (x fastest)."""
+        return _dense_export(lambda pts, cnt, cap, n: self.L.loam_b200_map_dense_export(self.h, pts, cnt, cap, n),
+                             self.dense_stats()["voxels"], lambda rc: self._ck(rc, "denseMap"))
+
+    def clear_dense_map(self):
+        self._ck(self.L.loam_b200_map_dense_clear(self.h), "clearDenseMap")
 
     def enable_sharding(self, rank, world, nccl_id: bytes | None):
         """Evaluate the rank-th of `world` query slices; with nccl_id (128 bytes, same on every rank) the normal

@@ -184,6 +184,8 @@ struct SortScratch {
   DevBuf<uint32_t> hist;
 };
 
+struct DenseMap;  // whole-run voxel map (densemap.cuh), created by loam_b200_dense_enable
+
 }  // namespace loamb
 
 // One helper thread per context for work whose ISSUE time (tens of launches) would otherwise sit on the caller's critical
@@ -367,6 +369,9 @@ struct loam_b200_ctx {
   loamb::DevBuf<uint32_t> vox_key;
   loamb::DevBuf<int> vox_val;
   loamb::DevBuf<int> vox_scalars;
+
+  // whole-run voxel map: null until enabled, so a context without it allocates and launches nothing for it
+  loamb::DenseMap* dense = nullptr;
 };
 
 namespace loamb {

@@ -1,0 +1,309 @@
+// Whole-run voxel map (optional, off by default): every registered full-resolution cloud the mapping stage produces is
+// accumulated into a device-resident open-addressing hash table of voxels that is never rolled or pruned -- the map of
+// the whole run, which the reference itself never keeps (its cube grid forgets cubes that roll out of the window).
+//
+// Voxel of a point: v_a = (int)floorf(c_a * (1.0f / leaf)) per axis, PCL VoxelGrid's index before it subtracts min_b
+// (voxel.cuh: voxel_key_of), so one cloud's voxels form the same partition as VoxelGrid.  Key = (v_z + 2^20) << 42 |
+// (v_y + 2^20) << 21 | (v_x + 2^20): z-major, so ascending keys are VoxelGrid's output order.  Points that are not
+// finite or whose voxel lies outside [-2^20, 2^20) on an axis are skipped (and counted).
+//
+// One insert of n points:
+//   key kernel -> stable two-pass LSD sort of the 64-bit keys (low word, then high word; radix_sort_pairs) -> run heads
+//   (voxel_head_kernel + radix_scan_kernel) -> one thread per run: sequential fp64 sums in ascending cloud index, and
+//   the run's slot if the voxel is already in the table -> block ranks of the new voxels in key order + scan ->
+//   insert (existing voxels add their partial sums, new ones are admitted in ascending key order while the table has
+//   room under max_voxels) -> counters.
+// Per voxel the table keeps count and the fp64 sums S = ((P1 + P2) + P3) + ... of the per-sweep partial sums; export
+// gives (float)(S / count) per field in ascending key order, so the result does not depend on where the hash placed
+// an entry.  Keys are unique within one insert, so no value update needs an atomic.
+#pragma once
+
+#include "voxel.cuh"
+
+namespace loamb {
+
+constexpr unsigned long long DENSE_EMPTY = ~0ull;  // empty table slot; also the key of a skipped point (sorts last)
+constexpr float DENSE_KEY_LIM = 1048576.f;          // 2^20 voxels per half axis
+
+struct __align__(16) DenseSlot {  // 48 B
+  unsigned long long key;
+  unsigned count;
+  unsigned pad;
+  double sum[4];                  // x, y, z, intensity
+};
+
+struct DenseCounters {
+  unsigned long long voxels, skipped, dropped;
+};
+
+// per-run results of one insert (indexed by run = voxel rank in key order)
+struct DenseRuns {
+  unsigned long long* key;
+  unsigned* count;
+  double4* sum;
+  long long* slot;  // table slot of a voxel already in the map, -1 new, -2 the run of skipped points
+};
+
+__device__ __forceinline__ unsigned long long dense_key_of(const float4& q, float inv) {
+  const float fx = floorf(q.x * inv), fy = floorf(q.y * inv), fz = floorf(q.z * inv);
+  // NaN fails every comparison; +-inf and out-of-range voxels fail the bounds (compared before the int conversion)
+  if (!(fx >= -DENSE_KEY_LIM && fx < DENSE_KEY_LIM && fy >= -DENSE_KEY_LIM && fy < DENSE_KEY_LIM &&
+        fz >= -DENSE_KEY_LIM && fz < DENSE_KEY_LIM))
+    return DENSE_EMPTY;
+  const unsigned long long vx = (unsigned long long)((int)fx + (1 << 20));
+  const unsigned long long vy = (unsigned long long)((int)fy + (1 << 20));
+  const unsigned long long vz = (unsigned long long)((int)fz + (1 << 20));
+  return (vz << 42) | (vy << 21) | vx;
+}
+
+// 64-bit finaliser of splitmix64: consecutive voxel keys spread over the whole table
+__device__ __forceinline__ unsigned long long dense_hash(unsigned long long k) {
+  k ^= k >> 30;
+  k *= 0xbf58476d1ce4e5b9ull;
+  k ^= k >> 27;
+  k *= 0x94d049bb133111ebull;
+  k ^= k >> 31;
+  return k;
+}
+
+__device__ __forceinline__ long long dense_find(const DenseSlot* __restrict__ t, unsigned long long mask,
+                                                unsigned long long key) {
+  unsigned long long h = dense_hash(key) & mask;
+  for (;;) {
+    const unsigned long long k = t[h].key;
+    if (k == key) return (long long)h;
+    if (k == DENSE_EMPTY) return -1;
+    h = (h + 1) & mask;
+  }
+}
+
+// claim an empty slot for `key` (absent from the table; load factor <= 0.5, so the probe ends)
+__device__ __forceinline__ unsigned long long dense_claim(DenseSlot* t, unsigned long long mask, unsigned long long key) {
+  unsigned long long h = dense_hash(key) & mask;
+  while (atomicCAS(&t[h].key, DENSE_EMPTY, key) != DENSE_EMPTY) h = (h + 1) & mask;
+  return h;
+}
+
+// 64-bit key per point + the (low word, index) pairs of the first sort pass
+__global__ void dense_key_kernel(const float4* __restrict__ p, int n, float inv, unsigned long long* __restrict__ keys64,
+                                 unsigned* __restrict__ keys_lo, int* __restrict__ vals) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long k = dense_key_of(p[i], inv);
+  keys64[i] = k;
+  keys_lo[i] = (unsigned)k;
+  vals[i] = i;
+}
+
+// export: the (low word, index) pairs of the compacted keys
+__global__ void dense_lo_kernel(const unsigned long long* __restrict__ keys64, int n, unsigned* __restrict__ keys_lo,
+                                int* __restrict__ vals) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  keys_lo[i] = (unsigned)keys64[i];
+  vals[i] = i;
+}
+
+// second pass input: high words in the order of the first pass (stable passes keep the index order inside a key)
+__global__ void dense_hi_kernel(const unsigned long long* __restrict__ keys64, const int* order, int n,
+                                unsigned* keys_hi, int* vals) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int o = order[i];  // order may alias vals: read before the write
+  keys_hi[i] = (unsigned)(keys64[o] >> 32);
+  vals[i] = o;
+}
+
+__global__ void dense_gather_keys_kernel(const unsigned long long* __restrict__ keys64, const int* __restrict__ order,
+                                         int n, unsigned long long* __restrict__ sorted) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) sorted[i] = keys64[order[i]];
+}
+
+// one thread per run head (sorted position i): the run's points in ascending cloud index, each float converted to
+// double and added in that order; then the voxel's slot if the table already holds it
+__global__ void dense_run_kernel(const float4* __restrict__ p, const unsigned long long* __restrict__ skey,
+                                 const int* __restrict__ order, const unsigned* __restrict__ pos,
+                                 const unsigned* __restrict__ block_off, int n, const DenseSlot* __restrict__ table,
+                                 unsigned long long mask, DenseRuns runs, DenseCounters* __restrict__ ctr) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned pv = pos[i];
+  if (!(pv >> 31)) return;
+  const unsigned r = (pv & 0x7fffffffu) + block_off[i / SCAN_BS];
+  const unsigned long long k = skey[i];
+  double sx = 0.0, sy = 0.0, sz = 0.0, si = 0.0;
+  unsigned cnt = 0;
+  for (int u = i; u < n && skey[u] == k; u++) {
+    const float4 q = p[order[u]];
+    sx += (double)q.x;
+    sy += (double)q.y;
+    sz += (double)q.z;
+    si += (double)q.w;
+    cnt++;
+  }
+  runs.key[r] = k;
+  runs.count[r] = cnt;
+  if (k == DENSE_EMPTY) {  // the skipped points: one run, the last
+    runs.slot[r] = -2;
+    ctr->skipped += cnt;
+    return;
+  }
+  runs.sum[r] = make_double4(sx, sy, sz, si);
+  runs.slot[r] = dense_find(table, mask, k);
+}
+
+// exclusive rank of every new voxel among the new voxels of its block (runs are in key order) + per-block totals
+__global__ void __launch_bounds__(SCAN_BS)
+dense_new_rank_kernel(const long long* __restrict__ slot, const int* __restrict__ n_runs, int bound,
+                      unsigned* __restrict__ rank, unsigned* __restrict__ block_sums) {
+  __shared__ unsigned ws[32];
+  const int r = blockIdx.x * SCAN_BS + threadIdx.x;
+  const int m = min(bound, *n_runs);
+  const unsigned f = (r < m && slot[r] == -1) ? 1u : 0u;
+  unsigned x = f;
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned y = __shfl_up_sync(0xffffffffu, x, o);
+    if ((threadIdx.x & 31) >= o) x += y;
+  }
+  if ((threadIdx.x & 31) == 31) ws[threadIdx.x >> 5] = x;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    unsigned w = ws[threadIdx.x];
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned y = __shfl_up_sync(0xffffffffu, w, o);
+      if (threadIdx.x >= o) w += y;
+    }
+    ws[threadIdx.x] = w;
+  }
+  __syncthreads();
+  const unsigned incl = x + ((threadIdx.x >> 5) ? ws[(threadIdx.x >> 5) - 1] : 0u);
+  if (r < bound) rank[r] = incl - f;
+  if (threadIdx.x == SCAN_BS - 1) block_sums[blockIdx.x] = incl;
+}
+
+// existing voxels add the run's partial sums; a new voxel is admitted when fewer than max_voxels - voxels new voxels
+// precede it in key order, otherwise its points are dropped.  ctr->voxels is read here and advanced by
+// dense_finish_kernel afterwards.
+__global__ void dense_insert_kernel(DenseRuns runs, const int* __restrict__ n_runs, const unsigned* __restrict__ rank,
+                                    const unsigned* __restrict__ block_off, DenseSlot* table, unsigned long long mask,
+                                    DenseCounters* __restrict__ ctr, unsigned long long max_voxels) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= *n_runs) return;
+  const long long s = runs.slot[r];
+  if (s == -2) return;
+  const double4 p = runs.sum[r];
+  const unsigned cnt = runs.count[r];
+  if (s >= 0) {
+    DenseSlot& e = table[s];
+    e.count += cnt;
+    e.sum[0] += p.x;
+    e.sum[1] += p.y;
+    e.sum[2] += p.z;
+    e.sum[3] += p.w;
+    return;
+  }
+  const unsigned long long nr = rank[r] + block_off[r / SCAN_BS];
+  if (ctr->voxels + nr >= max_voxels) {
+    atomicAdd(&ctr->dropped, (unsigned long long)cnt);
+    return;
+  }
+  DenseSlot& e = table[dense_claim(table, mask, runs.key[r])];
+  e.count = cnt;
+  e.sum[0] = p.x;
+  e.sum[1] = p.y;
+  e.sum[2] = p.z;
+  e.sum[3] = p.w;
+}
+
+__global__ void dense_finish_kernel(DenseCounters* ctr, const int* __restrict__ new_total, unsigned long long max_voxels) {
+  if (threadIdx.x != 0) return;
+  // the cap may have been lowered below the stored voxels (loam_b200_dense_enable): then no room at all
+  const unsigned long long room = ctr->voxels < max_voxels ? max_voxels - ctr->voxels : 0ull;
+  const unsigned long long nt = (unsigned long long)*new_total;
+  ctr->voxels += nt < room ? nt : room;
+}
+
+// growth: every entry of the old table moves to the new one (each key once, so a plain claim suffices)
+__global__ void dense_rehash_kernel(const DenseSlot* __restrict__ old_t, unsigned long long old_size, DenseSlot* t,
+                                   unsigned long long mask) {
+  const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
+  if (i >= old_size) return;
+  const DenseSlot e = old_t[i];
+  if (e.key == DENSE_EMPTY) return;
+  t[dense_claim(t, mask, e.key)] = e;
+}
+
+// export: occupied slots -> (key, slot) in any order (sorted by key afterwards); at most cap are written, the counter
+// counts them all (the caller checks it against the voxel counter)
+__global__ void dense_compact_kernel(const DenseSlot* __restrict__ t, unsigned long long size,
+                                     unsigned long long* __restrict__ keys, int* __restrict__ slots,
+                                     unsigned* __restrict__ counter, unsigned cap) {
+  const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
+  if (i >= size) return;
+  const unsigned long long k = t[i].key;
+  if (k == DENSE_EMPTY) return;
+  const unsigned d = atomicAdd(counter, 1u);
+  if (d >= cap) return;
+  keys[d] = k;
+  slots[d] = (int)i;
+}
+
+__global__ void dense_centroid_kernel(const DenseSlot* __restrict__ t, const int* __restrict__ slots,
+                                      const int* __restrict__ order, int m, float4* __restrict__ out,
+                                      unsigned* __restrict__ counts) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const DenseSlot& e = t[slots[order[i]]];
+  const double c = (double)e.count;
+  out[i] = make_float4((float)(e.sum[0] / c), (float)(e.sum[1] / c), (float)(e.sum[2] / c), (float)(e.sum[3] / c));
+  if (counts) counts[i] = e.count;
+}
+
+// Host-side state of the map (loam_b200_ctx::dense).  The insertion runs on its own stream with its own sort scratch,
+// so the next sweep's stages on the main stream and the map update on its lanes neither wait for it nor share buffers.
+struct DenseMap {
+  float leaf = 0.f;
+  unsigned long long max_voxels = 0;
+  cudaStream_t stream = nullptr;
+  cudaEvent_t ev_in = nullptr;    // the cloud is complete (main stream)
+  cudaEvent_t ev_done = nullptr;  // the last insertion has read its cloud (and mirrored the counters to ctr_host)
+  unsigned pending_slots = 0;     // cloud slots an insertion may still read: the next write waits for ev_done
+  SortScratch sort;
+  DevBuf<unsigned long long> keys64, skeys;
+  DevBuf<unsigned> pos, rank;
+  DevBuf<unsigned long long> run_key;
+  DevBuf<unsigned> run_count;
+  DevBuf<double4> run_sum;
+  DevBuf<long long> run_slot;
+  DevBuf<int> slots, ints;        // export: slot of each compacted voxel; [0] runs, [1] new voxels, [2] compaction counter
+  DevBuf<float4> out;
+  DevBuf<unsigned> out_count;
+  DevBuf<DenseCounters> ctr;
+  PinBuf<DenseCounters> ctr_host;
+  DenseSlot* table = nullptr;     // stream-ordered allocation (cudaMallocAsync on `stream`)
+  unsigned long long table_size = 0;
+  unsigned long long bound = 0;   // upper bound of the voxels in the table, known without a readback
+
+  // stream, events and buffers (the map's own; the context's stream must not be inside a DenseScope)
+  void release() {
+    if (stream) {
+      cudaStreamSynchronize(stream);
+      if (table) cudaFreeAsync(table, stream);
+      cudaStreamSynchronize(stream);
+      cudaStreamDestroy(stream);
+    }
+    stream = nullptr;
+    table = nullptr;
+    table_size = 0;
+    sort.keys_a.release(); sort.keys_b.release(); sort.vals_a.release(); sort.vals_b.release(); sort.hist.release();
+    keys64.release(); skeys.release(); pos.release(); rank.release(); run_key.release(); run_count.release();
+    run_sum.release(); run_slot.release(); slots.release(); ints.release(); out.release(); out_count.release();
+    ctr.release(); ctr_host.release();
+    if (ev_in) cudaEventDestroy(ev_in);
+    if (ev_done) cudaEventDestroy(ev_done);
+    ev_in = ev_done = nullptr;
+  }
+};
+
+}  // namespace loamb

@@ -89,6 +89,30 @@ void BasicLaserMapping::retainFromMapClouds(bool on) {
   _gpu->check(loam_b200_map_debug_from_map(_gpu->get(), on ? 1 : 0), "loam_b200_map_debug_from_map");
 }
 
+void BasicLaserMapping::enableDenseMap(float leaf, long long maxVoxels) {
+  _gpu->check(loam_b200_dense_enable(_gpu->get(), leaf, maxVoxels), "loam_b200_dense_enable");
+}
+
+BasicLaserMapping::DenseMapStats BasicLaserMapping::denseMapStats() {
+  long long s[3] = {0, 0, 0};
+  _gpu->check(loam_b200_dense_stats(_gpu->get(), s), "loam_b200_dense_stats");
+  return DenseMapStats{s[0], s[1], s[2]};
+}
+
+void BasicLaserMapping::denseMap(Cloud& out, std::vector<uint32_t>* counts) {
+  const int n = (int)denseMapStats().voxels;
+  std::vector<float> buf((size_t)n * 4 + 4);
+  if (counts) counts->resize((size_t)n);
+  int got = 0;
+  _gpu->check(loam_b200_dense_export(_gpu->get(), buf.data(), counts && n > 0 ? counts->data() : nullptr, n, &got),
+              "loam_b200_dense_export");
+  b200::unpack(buf.data(), (size_t)got, out);
+}
+
+void BasicLaserMapping::clearDenseMap() {
+  _gpu->check(loam_b200_dense_clear(_gpu->get()), "loam_b200_dense_clear");
+}
+
 void BasicLaserMapping::adopt(BasicLaserOdometry& odom) {
   static const int to[3] = {M_CORNER_LAST, M_SURF_LAST, M_FULL};
   int dstSlots[3], srcSlots[3];

@@ -86,9 +86,11 @@ struct OdomH {
     return which == 0 ? *o.lastCornerCloud() : which == 1 ? *o.lastSurfaceCloud() : o.deviceCloud(2).host();
   }
 };
+struct StreamRunner;
 struct MapH {
   loam::BasicLaserMapping m;
   Cloud scratchA, scratchB;
+  StreamRunner* runner = nullptr;  // the pipeline's stage threads when this is a streaming pipeline's mapping object
   MapH(float sp, int it) : m(sp, it) {}
   const Cloud& cloud(int which) {
     switch (which) {
@@ -103,7 +105,6 @@ struct MapH {
     }
   }
 };
-struct StreamRunner;
 struct PipeH {
   RegH reg;
   OdomH odom;
@@ -140,7 +141,7 @@ struct StreamRunner {
   std::condition_variable cv;
   std::deque<SweepJob> in;
   std::deque<SweepResult> out;
-  long next_id = 0, reg_done = 0, odom_done = 0, n_submitted = 0, n_finished = 0;
+  long next_id = 0, reg_done = 0, odom_done = 0, n_submitted = 0, n_finished = 0, n_collected = 0;
   bool reg_ready = false, odom_ready = false, stop = false;
   std::string err;
   // seconds each stage spent working / waiting for its neighbours (loam_b200_pipeline_stage_seconds)
@@ -351,6 +352,11 @@ struct StreamRunner {
     cv.notify_all();
     return 0;
   }
+  // a sweep is in flight from its submit() until its result has been collected
+  bool in_flight() {
+    std::lock_guard<std::mutex> lk(m);
+    return n_collected != n_submitted;
+  }
   // 1 = a result was returned, 0 = none pending / none ready (wait == 0), -1 = a stage failed
   int collect(int wait, SweepResult* r) {
     std::unique_lock<std::mutex> lk(m);
@@ -358,6 +364,7 @@ struct StreamRunner {
     if (!out.empty()) {
       *r = out.front();
       out.pop_front();
+      n_collected++;
       return 1;
     }
     if (!err.empty()) { g_err = err; return -1; }
@@ -366,6 +373,13 @@ struct StreamRunner {
 };
 
 PipeH::~PipeH() { delete runner; }
+
+// the mapping object of a streaming pipeline belongs to its stage thread while sweeps are in flight
+int map_in_flight(MapH* h) {
+  if (!h->runner || !h->runner->in_flight()) return 0;
+  g_err = "the pipeline has sweeps in flight (submitted, result not collected yet): collect them first";
+  return LOAM_B200_ERR_STATE;
+}
 
 }  // namespace
 
@@ -497,6 +511,36 @@ int loam_b200_map_cloud_copy(void* h, int which, float* out) { dump(((MapH*)h)->
 int loam_b200_map_last_iterations(void* h) { return (int)((MapH*)h)->m.lastIterationCount(); }
 int loam_b200_map_retain_from_map(void* h, int on) {
   return guarded([&] { ((MapH*)h)->m.retainFromMapClouds(on != 0); return 0; });
+}
+int loam_b200_map_dense_enable(void* h, float leaf, long long max_voxels) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  return guarded([&] { ((MapH*)h)->m.enableDenseMap(leaf, max_voxels); return 0; });
+}
+int loam_b200_map_dense_stats(void* h, long long* out3) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  return guarded([&] {
+    const auto s = ((MapH*)h)->m.denseMapStats();
+    out3[0] = s.voxels; out3[1] = s.skipped; out3[2] = s.dropped;
+    return 0;
+  });
+}
+int loam_b200_map_dense_export(void* h, float* xyzi, unsigned int* counts, int cap, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    std::vector<uint32_t> cnt;
+    m->m.denseMap(m->scratchA, counts ? &cnt : nullptr);
+    const int n = (int)m->scratchA.points.size();
+    *n_out = n;
+    if (n > cap) { g_err = "loam_b200_map_dense_export: output capacity too small"; return (int)LOAM_B200_ERR_CAPACITY; }
+    dump(m->scratchA, xyzi);
+    if (counts && n > 0) std::memcpy(counts, cnt.data(), (size_t)n * sizeof(uint32_t));
+    return 0;
+  });
+}
+int loam_b200_map_dense_clear(void* h) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  return guarded([&] { ((MapH*)h)->m.clearDenseMap(); return 0; });
 }
 int loam_b200_map_last_phase_seconds(void* h, double* out4) {
   const double* p = ((MapH*)h)->m.lastPhaseSeconds();
@@ -702,7 +746,10 @@ int loam_b200_pipeline_sync(void* hh) {
 int loam_b200_pipeline_submit(void* hh, const float* pts, const void* d_pts, const int* ring_sizes, int n_rings) {
   PipeH* h = (PipeH*)hh;
   if (!h || (!pts && !d_pts) || !ring_sizes || n_rings <= 0) { g_err = "invalid argument"; return -1; }
-  if (!h->runner) h->runner = new StreamRunner(h);
+  if (!h->runner) {
+    h->runner = new StreamRunner(h);
+    h->map.runner = h->runner;
+  }
   return h->runner->submit(pts, d_pts, ring_sizes, n_rings);
 }
 

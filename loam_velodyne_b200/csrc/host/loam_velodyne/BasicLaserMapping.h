@@ -7,6 +7,7 @@
 // reduction per iteration; the host keeps the 6x6 solve and the O(1) pose algebra.
 #pragma once
 
+#include <cstdint>
 #include <vector>
 
 #include <pcl/filters/voxel_grid.h>
@@ -107,6 +108,18 @@ class BasicLaserMapping {
    *  _laserCloudCornerFromMap / _laserCloudSurfFromMap) after every process(); off by default, the persistent GPU map
    *  only needs their sizes. */
   void retainFromMapClouds(bool on);
+
+  // extension (not in the reference API): the whole-run voxel map.  Once enabled, every process() that returns true adds
+  // the registered full-resolution cloud (laserCloud() in the map frame) to a voxel map on the GPU that is never rolled
+  // or pruned, unlike the 21 x 11 x 21 cube grid.  Per voxel: point count and the centroid of x, y, z and intensity
+  // (fp64 sums), exported in ascending voxel order (pcl::VoxelGrid's order: x fastest, then y, then z).  At most
+  // maxVoxels voxels are kept: once full, new voxels are refused (their points counted as dropped) while the kept ones
+  // keep accumulating.  Off by default; throws on a sharded object and on another leaf while the map holds voxels.
+  struct DenseMapStats { long long voxels, skipped, dropped; };
+  void enableDenseMap(float leaf, long long maxVoxels = 2147483647ll);
+  DenseMapStats denseMapStats();
+  void denseMap(pcl::PointCloud<pcl::PointXYZI>& out, std::vector<uint32_t>* counts = nullptr);
+  void clearDenseMap();
 
  private:
   typedef pcl::PointCloud<pcl::PointXYZI> Cloud;

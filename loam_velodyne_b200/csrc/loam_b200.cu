@@ -14,6 +14,7 @@
 #include "clustersort.cuh"
 #include "mapstore.cuh"
 #include "frontend.cuh"
+#include "densemap.cuh"
 
 using namespace loamb;
 
@@ -669,6 +670,11 @@ int loam_b200_destroy(loam_b200_ctx* c) {
   async_shutdown(c);
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
+  if (c->dense) {
+    c->dense->release();
+    delete c->dense;
+    c->dense = nullptr;
+  }
   c->reg_pts.release(); c->reg_ring_start.release(); c->reg_ring_end.release(); c->reg_picks.release();
   c->reg_counts.release(); c->reg_label.release(); c->reg_lessflat.release(); c->stage.release(); c->stage2.release();
   for (auto& t : c->tree) {
@@ -759,6 +765,7 @@ int loam_b200_sync(loam_b200_ctx* c) {
   LB_CUDA(c, cudaStreamSynchronize(c->stream));
   for (auto& l : c->lanes)
     if (l.stream) LB_CUDA(c, cudaStreamSynchronize(l.stream));
+  if (c->dense) LB_CUDA(c, cudaStreamSynchronize(c->dense->stream));  // whole-run map insertion
   if (c->aux) return loam_b200_sync(c->aux);  // asynchronous surround cloud
   return LOAM_B200_OK;
 }

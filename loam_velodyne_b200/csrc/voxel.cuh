@@ -12,10 +12,12 @@ namespace loamb {
 int radix_sort_pairs(loam_b200_ctx* c, int m, int key_bits, unsigned** keys_out = nullptr, int** vals_out = nullptr,
                      const int* n_dev = nullptr);
 
-// heads[i] = 1 when sorted key i starts a run; per-block totals for the scan
+// heads[i] = 1 when sorted key i starts a run; per-block totals for the scan (32-bit voxel keys; 64-bit keys of the
+// whole-run map, densemap.cuh)
 constexpr int SCAN_BS = 1024;
+template <typename K>
 __global__ void __launch_bounds__(SCAN_BS)
-voxel_head_kernel(const unsigned* __restrict__ keys, int n, unsigned* __restrict__ pos, unsigned* __restrict__ block_sums) {
+voxel_head_kernel(const K* __restrict__ keys, int n, unsigned* __restrict__ pos, unsigned* __restrict__ block_sums) {
   __shared__ unsigned ws[32];
   const int i = blockIdx.x * SCAN_BS + threadIdx.x;
   const unsigned h = (i < n && (i == 0 || keys[i] != keys[i - 1])) ? 1u : 0u;

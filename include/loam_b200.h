@@ -365,12 +365,41 @@ int loam_b200_debug_tree_build_path(loam_b200_ctx* ctx, int slot);
  *   export: every voxel as packed float[4] centroids (+ counts when counts != NULL); *n_out = number of voxels,
  *           LOAM_B200_ERR_CAPACITY when it exceeds cap (synchronises).  Not enabled: an empty map.
  *   clear:  empty the map (the leaf may then change).
+ * Every voxel also keeps two 16-bit evidence counters that saturate at 65535: hits (inserts that put points into it;
+ * counted always) and misses (sweeps of the optional visibility pass that saw through it).  They never change the
+ * export above.  The visibility pass (off by default; DESIGN.md "Visibility pass") removes moving-object trails:
+ *   visibility: h_res_deg, v_res_deg (range-image pixel size) and margin (metres).  Each mapped sweep k, before its
+ *           insertion and on the map's stream: with the optimised pose, every finite point of MAP_FULL and every stored
+ *           voxel centroid (fp64 sum / count) go to the sensor frame in double (pointAssociateTobeMapped,
+ *           BasicLaserMapping.cpp:223-231, with double cos / sin of the negated float angles): range
+ *           r = sqrt((x*x + y*y) + z*z), elevation atan2(y, sqrt(x*x + z*z)), azimuth atan2(x, z);
+ *           row = clamp(floor((deg(elevation) + 90) / v_res), 0, rows - 1), rows = ceil(180 / v_res);
+ *           col = floor((deg(azimuth) + 180) / h_res) mod cols (non-negative), cols = ceil(360 / h_res).  Each pixel
+ *           holds the minimum (float) r of the sweep's points with r > 0; a stored voxel whose pixel holds a finite
+ *           value v with (double) v > r + margin gets one miss.  Pixels without a return are no evidence.  Cost: one
+ *           pass over every table slot per mapped sweep.  h_res_deg == 0 turns it off; non-finite values, h_res
+ *           outside (0, 360], v_res outside (0, 180], margin < 0 or rows * cols > 2^24 give LOAM_B200_ERR_ARG; without
+ *           the map (or on a sharded context) LOAM_B200_ERR_STATE.
+ *   observe: the pass over the cloud in any slot (map frame) seen from `pose` (kernel-level use and tests; the mapping
+ *           stage observes MAP_FULL itself); everything enqueued on the context afterwards waits for it.
+ *           LOAM_B200_ERR_STATE while the pass is off.
+ *   export_filtered: the voxels with (double) misses <= max_miss_ratio * (double) hits (max_miss_ratio >= 0; +inf
+ *           keeps every voxel and equals loam_b200_dense_export), in ascending voxel order, with the same centroids;
+ *           counts, hits and misses may each be NULL.  *n_out = number of voxels kept, LOAM_B200_ERR_CAPACITY when it
+ *           exceeds cap (synchronises).
  * ------------------------------------------------------------------------------------------------------------------ */
 int loam_b200_dense_enable(loam_b200_ctx* ctx, float leaf, long long max_voxels);
 int loam_b200_dense_insert(loam_b200_ctx* ctx, int slot);
 int loam_b200_dense_stats(loam_b200_ctx* ctx, long long out3[3]);
 int loam_b200_dense_export(loam_b200_ctx* ctx, float* xyzi, uint32_t* counts, int cap, int* n_out);
 int loam_b200_dense_clear(loam_b200_ctx* ctx);
+int loam_b200_dense_visibility(loam_b200_ctx* ctx, double h_res_deg, double v_res_deg, double margin);
+int loam_b200_dense_observe(loam_b200_ctx* ctx, int slot, const loam_b200_pose* pose);
+int loam_b200_dense_export_filtered(loam_b200_ctx* ctx, double max_miss_ratio, float* xyzi, uint32_t* counts,
+                                    uint16_t* hits, uint16_t* misses, int cap, int* n_out);
+/* Test query: slots of the map's hash table as the host sized it last (0 while the map is off).  The table keeps a
+ * load factor <= 0.5 of an upper bound of the voxels, so it follows the voxels stored, not the points inserted. */
+int loam_b200_debug_dense_table_slots(loam_b200_ctx* ctx, long long* out);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice

@@ -100,6 +100,14 @@ int loam_b200_map_dense_enable(void* h, float leaf, long long max_voxels);
 int loam_b200_map_dense_stats(void* h, long long* out3);
 int loam_b200_map_dense_export(void* h, float* xyzi, unsigned int* counts, int cap, int* n_out);
 int loam_b200_map_dense_clear(void* h);
+/* visibility pass (BasicLaserMapping::enableDenseVisibility, include/loam_b200.h "loam_b200_dense_visibility") and the
+ * export filtered by max_miss_ratio (BasicLaserMapping::denseMapFiltered): as loam_b200_map_dense_export,
+ * plus per-voxel hits / misses when non-NULL.  Same in-flight rule as the four above. */
+int loam_b200_map_dense_visibility(void* h, double h_res_deg, double v_res_deg, double margin);
+int loam_b200_map_dense_export_filtered(void* h, double max_miss_ratio, float* xyzi, unsigned int* counts,
+                                        unsigned short* hits, unsigned short* misses, int cap, int* n_out);
+/* test query: loam_b200_debug_dense_table_slots of the mapping object's context (BasicLaserMapping::denseTableSlots) */
+int loam_b200_map_debug_dense_table_slots(void* h, long long* out);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank
  * then enables sharding on its mapping object (nccl_id128 = NULL: slice the queries only, no collective) */
 int loam_b200_host_nccl_unique_id(unsigned char* out128);

@@ -11,6 +11,7 @@ compute call raises ``LoamB200Error``.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 
 import numpy as np
@@ -81,6 +82,7 @@ BUILD_NONE, BUILD_CLUSTER_PAIR, BUILD_CLUSTER, BUILD_MULTI_LAUNCH = range(4)
 K_FEATURES, K_TREE_BUILD, K_KNN, K_MAP_ITER, K_ODOM_ITER, K_TRANSFORM, K_VOXEL, K_DENSE = range(8)
 KERNEL_FAMILIES = ["features", "tree_build", "knn", "map_iter", "odom_iter", "transform", "voxel", "dense"]
 _U = C.POINTER(C.c_uint32)
+_U16 = C.POINTER(C.c_uint16)
 _LL = C.POINTER(C.c_longlong)
 DENSE_MAX_VOXELS = 2**31 - 1  # default cap of the whole-run voxel map: none below the export's int32 count
 
@@ -160,6 +162,10 @@ def lib():
         "loam_b200_dense_stats": (C.c_int, [vp, _LL]),
         "loam_b200_dense_export": (C.c_int, [vp, _F, _U, C.c_int, _I]),
         "loam_b200_dense_clear": (C.c_int, [vp]),
+        "loam_b200_dense_visibility": (C.c_int, [vp, C.c_double, C.c_double, C.c_double]),
+        "loam_b200_dense_observe": (C.c_int, [vp, C.c_int, C.POINTER(Pose)]),
+        "loam_b200_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
+        "loam_b200_debug_dense_table_slots": (C.c_int, [vp, _LL]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -208,6 +214,9 @@ def lib():
         "loam_b200_map_dense_stats": (C.c_int, [vp, _LL]),
         "loam_b200_map_dense_export": (C.c_int, [vp, _F, _U, C.c_int, _I]),
         "loam_b200_map_dense_clear": (C.c_int, [vp]),
+        "loam_b200_map_dense_visibility": (C.c_int, [vp, C.c_double, C.c_double, C.c_double]),
+        "loam_b200_map_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
+        "loam_b200_map_debug_dense_table_slots": (C.c_int, [vp, _LL]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_map_kernel_profile": (C.c_int, [vp, C.c_int, _D]),
@@ -571,10 +580,32 @@ class Ctx:
         self._ck(self.L.loam_b200_dense_stats(self.h, out.ctypes.data_as(_LL)), "dense_stats")
         return _dense_stats(out)
 
-    def dense_export(self):
-        """(centroids N x 4 float32, counts N uint32) in ascending voxel order."""
-        return _dense_export(lambda pts, cnt, cap, n: self.L.loam_b200_dense_export(self.h, pts, cnt, cap, n),
-                             self.dense_stats()["voxels"], lambda rc: self._ck(rc, "dense_export"))
+    def dense_export(self, max_miss_ratio=None, evidence=False):
+        """(centroids N x 4 float32, counts N uint32) in ascending voxel order.  With max_miss_ratio only the voxels with
+        misses <= max_miss_ratio * hits; with evidence=True also (hits N uint16, misses N uint16)."""
+        if max_miss_ratio is None and not evidence:
+            return _dense_export(lambda pts, cnt, cap, n: self.L.loam_b200_dense_export(self.h, pts, cnt, cap, n),
+                                 self.dense_stats()["voxels"], lambda rc: self._ck(rc, "dense_export"))
+        return _dense_export_filtered(
+            lambda *a: self.L.loam_b200_dense_export_filtered(self.h, *a), max_miss_ratio, evidence,
+            self.dense_stats()["voxels"], lambda rc: self._ck(rc, "dense_export_filtered"))
+
+    def dense_table_slots(self):
+        """Test query: slots of the whole-run map's hash table (0 while the map is off)."""
+        out = C.c_longlong(0)
+        self._ck(self.L.loam_b200_debug_dense_table_slots(self.h, C.byref(out)), "dense_table_slots")
+        return out.value
+
+    def dense_visibility(self, h_res_deg, v_res_deg, margin):
+        """Visibility pass of every later insert by the mapping stage (h_res_deg = 0: off); see dense_observe."""
+        self._ck(self.L.loam_b200_dense_visibility(self.h, float(h_res_deg), float(v_res_deg), float(margin)),
+                 "dense_visibility")
+
+    def dense_observe(self, slot, twist6):
+        """The visibility pass over the cloud in `slot` (map frame) seen from the pose (rot_x, rot_y, rot_z, x, y, z):
+        one miss for every stored voxel the cloud sees through."""
+        p = make_pose(twist6)
+        self._ck(self.L.loam_b200_dense_observe(self.h, slot, C.byref(p)), "dense_observe")
 
     def dense_clear(self):
         self._ck(self.L.loam_b200_dense_clear(self.h), "dense_clear")
@@ -606,6 +637,20 @@ def _dense_export(fn, n, ck):
     got = C.c_int(0)
     ck(fn(_fp(pts), cnt.ctypes.data_as(_U), n, C.byref(got)))
     return pts[:got.value].copy(), cnt[:got.value].copy()
+
+
+def _dense_export_filtered(fn, max_miss_ratio, evidence, n, ck):
+    ratio = math.inf if max_miss_ratio is None else float(max_miss_ratio)
+    pts = np.zeros((max(n, 1), 4), np.float32)
+    cnt = np.zeros(max(n, 1), np.uint32)
+    hits = np.zeros(max(n, 1), np.uint16)
+    misses = np.zeros(max(n, 1), np.uint16)
+    got = C.c_int(0)
+    ck(fn(ratio, _fp(pts), cnt.ctypes.data_as(_U), hits.ctypes.data_as(_U16) if evidence else None,
+          misses.ctypes.data_as(_U16) if evidence else None, n, C.byref(got)))
+    k = got.value
+    out = (pts[:k].copy(), cnt[:k].copy())
+    return out + (hits[:k].copy(), misses[:k].copy()) if evidence else out
 
 
 def _ne(ne: NormalEq):
@@ -771,10 +816,28 @@ class LaserMapping(_Handle):
         self._ck(self.L.loam_b200_map_dense_stats(self.h, out.ctypes.data_as(_LL)), "denseMapStats")
         return _dense_stats(out)
 
-    def dense_map(self):
-        """(centroids N x 4 float32: x, y, z, intensity; counts N uint32) in ascending voxel order (x fastest)."""
-        return _dense_export(lambda pts, cnt, cap, n: self.L.loam_b200_map_dense_export(self.h, pts, cnt, cap, n),
-                             self.dense_stats()["voxels"], lambda rc: self._ck(rc, "denseMap"))
+    def dense_map(self, max_miss_ratio=None, evidence=False):
+        """(centroids N x 4 float32: x, y, z, intensity; counts N uint32) in ascending voxel order (x fastest).  With
+        max_miss_ratio only the voxels with misses <= max_miss_ratio * hits; with evidence=True also (hits N uint16,
+        misses N uint16)."""
+        if max_miss_ratio is None and not evidence:
+            return _dense_export(lambda pts, cnt, cap, n: self.L.loam_b200_map_dense_export(self.h, pts, cnt, cap, n),
+                                 self.dense_stats()["voxels"], lambda rc: self._ck(rc, "denseMap"))
+        return _dense_export_filtered(
+            lambda *a: self.L.loam_b200_map_dense_export_filtered(self.h, *a), max_miss_ratio, evidence,
+            self.dense_stats()["voxels"], lambda rc: self._ck(rc, "denseMap"))
+
+    def dense_table_slots(self):
+        """Test query: slots of the whole-run map's hash table (0 while the map is off)."""
+        out = C.c_longlong(0)
+        self._ck(self.L.loam_b200_map_debug_dense_table_slots(self.h, C.byref(out)), "denseTableSlots")
+        return out.value
+
+    def enable_dense_visibility(self, h_res_deg, v_res_deg, margin):
+        """Count, per voxel of the whole-run map, the mapped sweeps that see through it (h_res_deg = 0: off); filter
+        with dense_map(max_miss_ratio=...)."""
+        self._ck(self.L.loam_b200_map_dense_visibility(self.h, float(h_res_deg), float(v_res_deg), float(margin)),
+                 "enableDenseVisibility")
 
     def clear_dense_map(self):
         self._ck(self.L.loam_b200_map_dense_clear(self.h), "clearDenseMap")

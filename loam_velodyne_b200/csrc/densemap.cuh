@@ -13,6 +13,9 @@
 //   the run's slot if the voxel is already in the table -> block ranks of the new voxels in key order + scan ->
 //   insert (existing voxels add their partial sums, new ones are admitted in ascending key order while the table has
 //   room under max_voxels) -> counters.
+// Every insert also counts a hit for each voxel that receives points.  The optional visibility pass (before a sweep's
+// insert, dense_range_image_kernel + dense_visibility_kernel) counts a miss for every stored voxel that the sweep sees
+// through: its pixel of the sweep's range image holds a return farther than the centroid's range + margin.
 // Per voxel the table keeps count and the fp64 sums S = ((P1 + P2) + P3) + ... of the per-sweep partial sums; export
 // gives (float)(S / count) per field in ascending key order, so the result does not depend on where the hash placed
 // an entry.  Keys are unique within one insert, so no value update needs an atomic.
@@ -28,9 +31,14 @@ constexpr float DENSE_KEY_LIM = 1048576.f;          // 2^20 voxels per half axis
 struct __align__(16) DenseSlot {  // 48 B
   unsigned long long key;
   unsigned count;
-  unsigned pad;
+  unsigned evidence;              // hits (low 16 bits) and misses (high 16 bits), each saturating at 65535
   double sum[4];                  // x, y, z, intensity
 };
+
+constexpr unsigned DENSE_EVIDENCE_NEW = 1u;  // a voxel's first insert: 1 hit, 0 misses
+
+__device__ __forceinline__ unsigned dense_add_hit(unsigned e) { return (e & 0xffffu) == 0xffffu ? e : e + 1u; }
+__device__ __forceinline__ unsigned dense_add_miss(unsigned e) { return (e >> 16) == 0xffffu ? e : e + 0x10000u; }
 
 struct DenseCounters {
   unsigned long long voxels, skipped, dropped;
@@ -197,6 +205,7 @@ __global__ void dense_insert_kernel(DenseRuns runs, const int* __restrict__ n_ru
   if (s >= 0) {
     DenseSlot& e = table[s];
     e.count += cnt;
+    e.evidence = dense_add_hit(e.evidence);
     e.sum[0] += p.x;
     e.sum[1] += p.y;
     e.sum[2] += p.z;
@@ -210,6 +219,7 @@ __global__ void dense_insert_kernel(DenseRuns runs, const int* __restrict__ n_ru
   }
   DenseSlot& e = table[dense_claim(table, mask, runs.key[r])];
   e.count = cnt;
+  e.evidence = DENSE_EVIDENCE_NEW;
   e.sum[0] = p.x;
   e.sum[1] = p.y;
   e.sum[2] = p.z;
@@ -234,16 +244,20 @@ __global__ void dense_rehash_kernel(const DenseSlot* __restrict__ old_t, unsigne
   t[dense_claim(t, mask, e.key)] = e;
 }
 
-// export: occupied slots -> (key, slot) in any order (sorted by key afterwards); at most cap are written, the counter
-// counts them all (the caller checks it against the voxel counter)
+// export: occupied slots -> counter[0]; those with (double)misses <= max_miss_ratio * (double)hits -> (key, slot) in any
+// order (sorted by key afterwards) and counter[1]; at most cap are written (the caller checks counter[0] against the
+// voxel counter).  max_miss_ratio = +inf keeps every voxel (hits >= 1 for every stored one).
 __global__ void dense_compact_kernel(const DenseSlot* __restrict__ t, unsigned long long size,
                                      unsigned long long* __restrict__ keys, int* __restrict__ slots,
-                                     unsigned* __restrict__ counter, unsigned cap) {
+                                     unsigned* __restrict__ counter, unsigned cap, double max_miss_ratio) {
   const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
   if (i >= size) return;
   const unsigned long long k = t[i].key;
   if (k == DENSE_EMPTY) return;
-  const unsigned d = atomicAdd(counter, 1u);
+  atomicAdd(&counter[0], 1u);
+  const unsigned ev = t[i].evidence;
+  if (!((double)(ev >> 16) <= max_miss_ratio * (double)(ev & 0xffffu))) return;
+  const unsigned d = atomicAdd(&counter[1], 1u);
   if (d >= cap) return;
   keys[d] = k;
   slots[d] = (int)i;
@@ -251,13 +265,82 @@ __global__ void dense_compact_kernel(const DenseSlot* __restrict__ t, unsigned l
 
 __global__ void dense_centroid_kernel(const DenseSlot* __restrict__ t, const int* __restrict__ slots,
                                       const int* __restrict__ order, int m, float4* __restrict__ out,
-                                      unsigned* __restrict__ counts) {
+                                      unsigned* __restrict__ counts, unsigned* __restrict__ evidence) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
   const DenseSlot& e = t[slots[order[i]]];
   const double c = (double)e.count;
   out[i] = make_float4((float)(e.sum[0] / c), (float)(e.sum[1] / c), (float)(e.sum[2] / c), (float)(e.sum[3] / c));
   if (counts) counts[i] = e.count;
+  if (evidence) evidence[i] = e.evidence;
+}
+
+// ---- visibility pass: one sweep's sensor pose and range image (include/loam_b200.h "loam_b200_dense_visibility")
+constexpr double DENSE_RAD2DEG = 180.0 / 3.14159265358979323846;
+constexpr unsigned DENSE_NO_RETURN = 0xffffffffu;  // empty pixel (above the bits of +inf, like every float bit pattern
+                                                   // of a non-negative float is below it)
+
+struct DenseView {                // by value in the kernel arguments
+  double px, py, pz;              // sensor position (the pose's float pos)
+  double cy, sy, cx, sx, cz, sz;  // cos / sin of -rot_y, -rot_x, -rot_z (double, computed by the host)
+  double h_res, v_res, margin;    // degrees, degrees, metres
+  int rows, cols;
+};
+
+// map-frame position -> range and pixel in the sensor frame of `v`, all in double: pointAssociateTobeMapped
+// (BasicLaserMapping.cpp:223-231: the offset, then rotY, rotX, rotZ of math_utils.h); elevation atan2(y, |(x, z)|)
+// (y up), azimuth atan2(x, z).  The library is built without FMA contraction, so every product and sum rounds on its
+// own, as in tests/visibility_reference.py.
+__device__ __forceinline__ int dense_pixel(const DenseView& v, double x, double y, double z, double& r) {
+  x -= v.px;
+  y -= v.py;
+  z -= v.pz;
+  double t = x;  // rotY
+  x = v.cy * t + v.sy * z;
+  z = v.cy * z - v.sy * t;
+  t = y;  // rotX
+  y = v.cx * t - v.sx * z;
+  z = v.sx * t + v.cx * z;
+  t = x;  // rotZ
+  x = v.cz * t - v.sz * y;
+  y = v.sz * t + v.cz * y;
+  r = sqrt((x * x + y * y) + z * z);
+  const double e = atan2(y, sqrt(x * x + z * z));
+  const double a = atan2(x, z);
+  const double fr = floor((e * DENSE_RAD2DEG + 90.0) / v.v_res);
+  const double fc = floor((a * DENSE_RAD2DEG + 180.0) / v.h_res);
+  const int row = fr < 0.0 ? 0 : (fr > (double)(v.rows - 1) ? v.rows - 1 : (int)fr);
+  int col = (int)((long long)fc % v.cols);
+  if (col < 0) col += v.cols;
+  return row * v.cols + col;
+}
+
+// one thread per point: the minimum range per pixel over the finite points with r > 0 (float bits of non-negative
+// floats order like the floats, so atomicMin gives the same image in any order)
+__global__ void dense_range_image_kernel(const float4* __restrict__ p, int n, DenseView v, unsigned* __restrict__ img) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 q = p[i];
+  if (!(isfinite(q.x) && isfinite(q.y) && isfinite(q.z))) return;
+  double r;
+  const int pix = dense_pixel(v, (double)q.x, (double)q.y, (double)q.z, r);
+  if (r > 0.0) atomicMin(&img[pix], __float_as_uint((float)r));
+}
+
+// one thread per table slot (grid-stride): a stored voxel whose pixel holds a finite return farther than its
+// centroid's range + margin is seen through -> one more miss.  Pixels without a return are no evidence.
+__global__ void dense_visibility_kernel(DenseSlot* t, unsigned long long size, DenseView v,
+                                        const unsigned* __restrict__ img) {
+  for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < size;
+       i += (unsigned long long)gridDim.x * blockDim.x) {
+    DenseSlot& e = t[i];
+    if (e.key == DENSE_EMPTY) continue;
+    const double c = (double)e.count;
+    double r;
+    const int pix = dense_pixel(v, e.sum[0] / c, e.sum[1] / c, e.sum[2] / c, r);
+    const unsigned b = img[pix];
+    if (b < 0x7f800000u && (double)__uint_as_float(b) > r + v.margin) e.evidence = dense_add_miss(e.evidence);
+  }
 }
 
 // Host-side state of the map (loam_b200_ctx::dense).  The insertion runs on its own stream with its own sort scratch,
@@ -268,6 +351,8 @@ struct DenseMap {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev_in = nullptr;    // the cloud is complete (main stream)
   cudaEvent_t ev_done = nullptr;  // the last insertion has read its cloud (and mirrored the counters to ctr_host)
+  cudaEvent_t ev_observed = nullptr;  // the last visibility pass has read its cloud (never ev_done: the insertion sizes
+                                      // the table from the counters only when ev_done says they are current)
   unsigned pending_slots = 0;     // cloud slots an insertion may still read: the next write waits for ev_done
   SortScratch sort;
   DevBuf<unsigned long long> keys64, skeys;
@@ -278,7 +363,10 @@ struct DenseMap {
   DevBuf<long long> run_slot;
   DevBuf<int> slots, ints;        // export: slot of each compacted voxel; [0] runs, [1] new voxels, [2] compaction counter
   DevBuf<float4> out;
-  DevBuf<unsigned> out_count;
+  DevBuf<unsigned> out_count, out_evidence;
+  double vis_h_res = 0.0, vis_v_res = 0.0, vis_margin = 0.0;  // visibility pass (vis_h_res == 0: off)
+  int vis_rows = 0, vis_cols = 0;
+  DevBuf<unsigned> image;         // range image of the sweep being observed (float bits, DENSE_NO_RETURN when empty)
   DevBuf<DenseCounters> ctr;
   PinBuf<DenseCounters> ctr_host;
   DenseSlot* table = nullptr;     // stream-ordered allocation (cudaMallocAsync on `stream`)
@@ -299,10 +387,12 @@ struct DenseMap {
     sort.keys_a.release(); sort.keys_b.release(); sort.vals_a.release(); sort.vals_b.release(); sort.hist.release();
     keys64.release(); skeys.release(); pos.release(); rank.release(); run_key.release(); run_count.release();
     run_sum.release(); run_slot.release(); slots.release(); ints.release(); out.release(); out_count.release();
+    out_evidence.release(); image.release();
     ctr.release(); ctr_host.release();
     if (ev_in) cudaEventDestroy(ev_in);
     if (ev_done) cudaEventDestroy(ev_done);
-    ev_in = ev_done = nullptr;
+    if (ev_observed) cudaEventDestroy(ev_observed);
+    ev_in = ev_done = ev_observed = nullptr;
   }
 };
 

@@ -109,6 +109,33 @@ void BasicLaserMapping::denseMap(Cloud& out, std::vector<uint32_t>* counts) {
   b200::unpack(buf.data(), (size_t)got, out);
 }
 
+void BasicLaserMapping::enableDenseVisibility(double hRes, double vRes, double margin) {
+  _gpu->check(loam_b200_dense_visibility(_gpu->get(), hRes, vRes, margin), "loam_b200_dense_visibility");
+}
+
+void BasicLaserMapping::denseMapFiltered(Cloud& out, double maxMissRatio, std::vector<uint32_t>* counts,
+                                         std::vector<uint16_t>* hits, std::vector<uint16_t>* misses) {
+  const int n = (int)denseMapStats().voxels;  // the voxels kept are a subset
+  std::vector<float> buf((size_t)n * 4 + 4);
+  if (counts) counts->resize((size_t)n + 1);
+  if (hits) hits->resize((size_t)n + 1);
+  if (misses) misses->resize((size_t)n + 1);
+  int got = 0;
+  _gpu->check(loam_b200_dense_export_filtered(_gpu->get(), maxMissRatio, buf.data(), counts ? counts->data() : nullptr,
+                                              hits ? hits->data() : nullptr, misses ? misses->data() : nullptr, n, &got),
+              "loam_b200_dense_export_filtered");
+  if (counts) counts->resize((size_t)got);
+  if (hits) hits->resize((size_t)got);
+  if (misses) misses->resize((size_t)got);
+  b200::unpack(buf.data(), (size_t)got, out);
+}
+
+long long BasicLaserMapping::denseTableSlots() {
+  long long n = 0;
+  _gpu->check(loam_b200_debug_dense_table_slots(_gpu->get(), &n), "loam_b200_debug_dense_table_slots");
+  return n;
+}
+
 void BasicLaserMapping::clearDenseMap() {
   _gpu->check(loam_b200_dense_clear(_gpu->get()), "loam_b200_dense_clear");
 }

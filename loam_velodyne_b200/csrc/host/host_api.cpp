@@ -538,6 +538,35 @@ int loam_b200_map_dense_export(void* h, float* xyzi, unsigned int* counts, int c
     return 0;
   });
 }
+int loam_b200_map_dense_visibility(void* h, double h_res_deg, double v_res_deg, double margin) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  return guarded([&] { ((MapH*)h)->m.enableDenseVisibility(h_res_deg, v_res_deg, margin); return 0; });
+}
+int loam_b200_map_dense_export_filtered(void* h, double max_miss_ratio, float* xyzi, unsigned int* counts,
+                                        unsigned short* hits, unsigned short* misses, int cap, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    std::vector<uint32_t> cnt;
+    std::vector<uint16_t> hit, miss;
+    m->m.denseMapFiltered(m->scratchA, max_miss_ratio, counts ? &cnt : nullptr, hits ? &hit : nullptr, misses ? &miss : nullptr);
+    const int n = (int)m->scratchA.points.size();
+    *n_out = n;
+    if (n > cap) {
+      g_err = "loam_b200_map_dense_export_filtered: output capacity too small";
+      return (int)LOAM_B200_ERR_CAPACITY;
+    }
+    dump(m->scratchA, xyzi);
+    if (counts && n > 0) std::memcpy(counts, cnt.data(), (size_t)n * sizeof(uint32_t));
+    if (hits && n > 0) std::memcpy(hits, hit.data(), (size_t)n * sizeof(uint16_t));
+    if (misses && n > 0) std::memcpy(misses, miss.data(), (size_t)n * sizeof(uint16_t));
+    return 0;
+  });
+}
+int loam_b200_map_debug_dense_table_slots(void* h, long long* out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  return guarded([&] { *out = ((MapH*)h)->m.denseTableSlots(); return 0; });
+}
 int loam_b200_map_dense_clear(void* h) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;
   return guarded([&] { ((MapH*)h)->m.clearDenseMap(); return 0; });

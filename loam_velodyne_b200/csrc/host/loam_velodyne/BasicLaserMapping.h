@@ -120,6 +120,18 @@ class BasicLaserMapping {
   DenseMapStats denseMapStats();
   void denseMap(pcl::PointCloud<pcl::PointXYZI>& out, std::vector<uint32_t>* counts = nullptr);
   void clearDenseMap();
+  // Visibility pass over the whole-run map (off by default; include/loam_b200.h "loam_b200_dense_visibility"): every
+  // process() first renders its registered cloud as a range image (hRes x vRes degree pixels, minimum range) from the
+  // optimised pose and counts a miss for every stored voxel that lies more than `margin` metres in front of the return
+  // in its pixel.  hRes = 0 turns it off; throws without the dense map and on bad arguments.
+  void enableDenseVisibility(double hRes, double vRes, double margin);
+  // the voxels with misses <= maxMissRatio * hits (a voxel's hits: the sweeps that put points into it); +inf returns
+  // every voxel, as denseMap above.  hits / misses: per-voxel evidence counters (saturating at 65535) when non-null.
+  void denseMapFiltered(pcl::PointCloud<pcl::PointXYZI>& out, double maxMissRatio,
+                        std::vector<uint32_t>* counts = nullptr, std::vector<uint16_t>* hits = nullptr,
+                        std::vector<uint16_t>* misses = nullptr);
+  /** Test hook (not in the reference): slots of the whole-run map's hash table (0 while the map is off). */
+  long long denseTableSlots();
 
  private:
   typedef pcl::PointCloud<pcl::PointXYZI> Cloud;

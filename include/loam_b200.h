@@ -387,6 +387,26 @@ int loam_b200_debug_tree_build_path(loam_b200_ctx* ctx, int slot);
  *           keeps every voxel and equals loam_b200_dense_export), in ascending voxel order, with the same centroids;
  *           counts, hits and misses may each be NULL.  *n_out = number of voxels kept, LOAM_B200_ERR_CAPACITY when it
  *           exceeds cap (synchronises).
+ *   export_normals: the export of export_filtered at max_miss_ratio (same voxels, order, centroids and counts, bit for
+ *           bit) plus a surface normal and curvature per voxel, computed over the exported voxels only (a voxel that
+ *           the filter removes gets no normal and is nobody's neighbour).  normals: float[4] (nx, ny, nz, curvature)
+ *           per voxel, in the centroids' order.  For voxel v with fp32 centroid c_v:
+ *             neighbours w: the exported voxels whose index differs from v's by at most `radius` (1..3) on every axis,
+ *               v included; an offset outside the key range [-2^20, 2^20) on an axis does not exist (never wraps into
+ *               the next row or plane of the key).  Visited in ascending key order (dz, then dy, then dx ascending).
+ *             fp64, no FMA, each operation rounded on its own: d = (double)c_w - (double)c_v per axis; S1 += d (3
+ *               components); S2 += d_a * d_b (xx, xy, xz, yy, yz, zz); k = number of neighbours;
+ *               C_ab = (float)((S2_ab - (S1_a * S1_b) / k) / k).
+ *             sym_eigen<3> of C (csrc/linalg.cuh, the 3x3 solver of the scan-to-map line fit): normal = eigenvector of
+ *               the smallest eigenvalue; curvature = ev0 / ((ev0 + ev1) + ev2) in fp32, 0 when that sum is 0.
+ *             orientation (pcl::flipNormalTowardsViewpoint): with p = viewpoint (map frame, double), the normal is
+ *               negated when ((p_x - c_x) * n_x + (p_y - c_y) * n_y) + (p_z - c_z) * n_z < 0 in double.
+ *             k < 3, or an eigen-decomposition that does not converge: NaN normal and curvature.
+ *           The result is pcl::NormalEstimation's on the exported cloud with a box neighbourhood, each neighbour's
+ *           centroid counted once (counts are no weights).  counts may be NULL; xyzi and normals may not once
+ *           voxels are exported.  *n_out and LOAM_B200_ERR_CAPACITY as export_filtered; LOAM_B200_ERR_ARG for radius
+ *           outside 1..3, a NaN or negative ratio, a NULL or non-finite viewpoint.  Runs only at export, never on the
+ *           per-sweep path.
  * ------------------------------------------------------------------------------------------------------------------ */
 int loam_b200_dense_enable(loam_b200_ctx* ctx, float leaf, long long max_voxels);
 int loam_b200_dense_insert(loam_b200_ctx* ctx, int slot);
@@ -397,6 +417,8 @@ int loam_b200_dense_visibility(loam_b200_ctx* ctx, double h_res_deg, double v_re
 int loam_b200_dense_observe(loam_b200_ctx* ctx, int slot, const loam_b200_pose* pose);
 int loam_b200_dense_export_filtered(loam_b200_ctx* ctx, double max_miss_ratio, float* xyzi, uint32_t* counts,
                                     uint16_t* hits, uint16_t* misses, int cap, int* n_out);
+int loam_b200_dense_export_normals(loam_b200_ctx* ctx, double max_miss_ratio, int radius, const double viewpoint[3],
+                                   float* xyzi, uint32_t* counts, float* normals, int cap, int* n_out);
 /* Test query: slots of the map's hash table as the host sized it last (0 while the map is off).  The table keeps a
  * load factor <= 0.5 of an upper bound of the voxels, so it follows the voxels stored, not the points inserted. */
 int loam_b200_debug_dense_table_slots(loam_b200_ctx* ctx, long long* out);

@@ -106,6 +106,11 @@ int loam_b200_map_dense_clear(void* h);
 int loam_b200_map_dense_visibility(void* h, double h_res_deg, double v_res_deg, double margin);
 int loam_b200_map_dense_export_filtered(void* h, double max_miss_ratio, float* xyzi, unsigned int* counts,
                                         unsigned short* hits, unsigned short* misses, int cap, int* n_out);
+/* the filtered export with a normal and curvature per voxel (BasicLaserMapping::denseMapNormals, include/loam_b200.h
+ * "loam_b200_dense_export_normals"): normals float[4] (nx, ny, nz, curvature) per voxel in the centroids' order; same
+ * arguments, capacity rule and in-flight rule as loam_b200_map_dense_export_filtered, viewpoint = 3 doubles. */
+int loam_b200_map_dense_export_normals(void* h, double max_miss_ratio, int radius, const double* viewpoint,
+                                       float* xyzi, unsigned int* counts, float* normals, int cap, int* n_out);
 /* test query: loam_b200_debug_dense_table_slots of the mapping object's context (BasicLaserMapping::denseTableSlots) */
 int loam_b200_map_debug_dense_table_slots(void* h, long long* out);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank

@@ -165,6 +165,7 @@ def lib():
         "loam_b200_dense_visibility": (C.c_int, [vp, C.c_double, C.c_double, C.c_double]),
         "loam_b200_dense_observe": (C.c_int, [vp, C.c_int, C.POINTER(Pose)]),
         "loam_b200_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
+        "loam_b200_dense_export_normals": (C.c_int, [vp, C.c_double, C.c_int, _D, _F, _U, _F, C.c_int, _I]),
         "loam_b200_debug_dense_table_slots": (C.c_int, [vp, _LL]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
@@ -216,6 +217,7 @@ def lib():
         "loam_b200_map_dense_clear": (C.c_int, [vp]),
         "loam_b200_map_dense_visibility": (C.c_int, [vp, C.c_double, C.c_double, C.c_double]),
         "loam_b200_map_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
+        "loam_b200_map_dense_export_normals": (C.c_int, [vp, C.c_double, C.c_int, _D, _F, _U, _F, C.c_int, _I]),
         "loam_b200_map_debug_dense_table_slots": (C.c_int, [vp, _LL]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
@@ -590,6 +592,14 @@ class Ctx:
             lambda *a: self.L.loam_b200_dense_export_filtered(self.h, *a), max_miss_ratio, evidence,
             self.dense_stats()["voxels"], lambda rc: self._ck(rc, "dense_export_filtered"))
 
+    def dense_export_normals(self, max_miss_ratio=None, radius=1, viewpoint=(0.0, 0.0, 0.0)):
+        """(centroids N x 4 float32, counts N uint32, normals N x 4 float32: nx, ny, nz, curvature) of the voxels
+        dense_export(max_miss_ratio) returns (None: every voxel).  Neighbourhood: the exported voxels within `radius`
+        (1..3) voxels on every axis; normals flipped towards `viewpoint` (map frame); NaN where fewer than 3 neighbours."""
+        return _dense_export_normals(lambda *a: self.L.loam_b200_dense_export_normals(self.h, *a), max_miss_ratio,
+                                     radius, viewpoint, self.dense_stats()["voxels"],
+                                     lambda rc: self._ck(rc, "dense_export_normals"))
+
     def dense_table_slots(self):
         """Test query: slots of the whole-run map's hash table (0 while the map is off)."""
         out = C.c_longlong(0)
@@ -651,6 +661,18 @@ def _dense_export_filtered(fn, max_miss_ratio, evidence, n, ck):
     k = got.value
     out = (pts[:k].copy(), cnt[:k].copy())
     return out + (hits[:k].copy(), misses[:k].copy()) if evidence else out
+
+
+def _dense_export_normals(fn, max_miss_ratio, radius, viewpoint, n, ck):
+    ratio = math.inf if max_miss_ratio is None else float(max_miss_ratio)
+    vp = np.ascontiguousarray(viewpoint, np.float64).reshape(3)
+    pts = np.zeros((max(n, 1), 4), np.float32)
+    cnt = np.zeros(max(n, 1), np.uint32)
+    nrm = np.zeros((max(n, 1), 4), np.float32)
+    got = C.c_int(0)
+    ck(fn(ratio, int(radius), vp.ctypes.data_as(_D), _fp(pts), cnt.ctypes.data_as(_U), _fp(nrm), n, C.byref(got)))
+    k = got.value
+    return pts[:k].copy(), cnt[:k].copy(), nrm[:k].copy()
 
 
 def _ne(ne: NormalEq):
@@ -826,6 +848,13 @@ class LaserMapping(_Handle):
         return _dense_export_filtered(
             lambda *a: self.L.loam_b200_map_dense_export_filtered(self.h, *a), max_miss_ratio, evidence,
             self.dense_stats()["voxels"], lambda rc: self._ck(rc, "denseMap"))
+
+    def dense_map_normals(self, max_miss_ratio=None, radius=1, viewpoint=(0.0, 0.0, 0.0)):
+        """(centroids N x 4, counts N, normals N x 4: nx, ny, nz, curvature) of the voxels dense_map(max_miss_ratio)
+        returns; see Ctx.dense_export_normals.  The default viewpoint, the origin, is the first sweep's sensor position."""
+        return _dense_export_normals(lambda *a: self.L.loam_b200_map_dense_export_normals(self.h, *a), max_miss_ratio,
+                                     radius, viewpoint, self.dense_stats()["voxels"],
+                                     lambda rc: self._ck(rc, "denseMapNormals"))
 
     def dense_table_slots(self):
         """Test query: slots of the whole-run map's hash table (0 while the map is off)."""

@@ -21,6 +21,7 @@
 // an entry.  Keys are unique within one insert, so no value update needs an atomic.
 #pragma once
 
+#include "linalg.cuh"
 #include "voxel.cuh"
 
 namespace loamb {
@@ -275,6 +276,97 @@ __global__ void dense_centroid_kernel(const DenseSlot* __restrict__ t, const int
   if (evidence) evidence[i] = e.evidence;
 }
 
+// ---- normals of the exported cloud (include/loam_b200.h "loam_b200_dense_export_normals")
+constexpr int DENSE_AXIS = 1 << 21;  // voxel indices per axis in the key (v + 2^20 in [0, 2^21))
+constexpr unsigned long long DENSE_AXIS_MASK = DENSE_AXIS - 1;
+
+// first position in [lo, hi) of the ascending keys whose key is >= `key`
+__device__ __forceinline__ int dense_lower_bound(const unsigned long long* __restrict__ k, int lo, int hi,
+                                                 unsigned long long key) {
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (k[mid] < key) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// One thread per exported voxel, over the export's own arrays (keys ascending, centroids in the same order), so the
+// miss-ratio filter is already applied and the table is never touched.  Neighbours: the exported voxels within `radius`
+// voxels on every axis, visited in ascending key order -- per (z, y) row inside the key range, a lower bound of the
+// row's first key (x clamped to the range), then forward while the key stays in the row.  Rows outside the range are
+// skipped, so an offset never wraps into the next row or plane.  Centred fp64 sums of the fp32 centroids, covariance
+// rounded to fp32 once per entry, sym_eigen<3>, curvature ev0 / (ev0 + ev1 + ev2), normal flipped towards the viewpoint.
+// Fewer than 3 neighbours, or no convergence: NaN normal and curvature.  The library is built without FMA contraction,
+// so every product and sum rounds on its own, as in tests/normals_reference.py.
+__global__ void __launch_bounds__(128)
+dense_normals_kernel(const unsigned long long* __restrict__ skey, const float4* __restrict__ cent, int n, int radius,
+                     double3 vp, float4* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long key = skey[i];
+  const int vx = (int)(key & DENSE_AXIS_MASK), vy = (int)((key >> 21) & DENSE_AXIS_MASK), vz = (int)(key >> 42);
+  const float4 cv = cent[i];
+  const double cx = (double)cv.x, cy = (double)cv.y, cz = (double)cv.z;
+  double s1x = 0.0, s1y = 0.0, s1z = 0.0, sxx = 0.0, sxy = 0.0, sxz = 0.0, syy = 0.0, syz = 0.0, szz = 0.0;
+  int k = 0;
+  const unsigned long long x0 = (unsigned long long)max(vx - radius, 0);
+  const unsigned long long x1 = (unsigned long long)min(vx + radius, DENSE_AXIS - 1);
+  int lo = 0;  // rows ascend in key order: each row's search starts where the previous row ended
+  for (int z = vz - radius; z <= vz + radius; z++) {
+    if (z < 0 || z >= DENSE_AXIS) continue;
+    for (int y = vy - radius; y <= vy + radius; y++) {
+      if (y < 0 || y >= DENSE_AXIS) continue;
+      const unsigned long long row = ((unsigned long long)z << 42) | ((unsigned long long)y << 21);
+      const unsigned long long last = row | x1;
+      int j = dense_lower_bound(skey, lo, n, row | x0);
+      for (; j < n && skey[j] <= last; j++) {
+        const float4 cw = cent[j];
+        const double dx = (double)cw.x - cx, dy = (double)cw.y - cy, dz = (double)cw.z - cz;
+        s1x += dx;
+        s1y += dy;
+        s1z += dz;
+        sxx += dx * dx;
+        sxy += dx * dy;
+        sxz += dx * dz;
+        syy += dy * dy;
+        syz += dy * dz;
+        szz += dz * dz;
+        k++;
+      }
+      lo = j;
+    }
+  }
+  const float qnan = __int_as_float(0x7fc00000);
+  if (k < 3) {
+    out[i] = make_float4(qnan, qnan, qnan, qnan);
+    return;
+  }
+  const double kd = (double)k;
+  float m[9];
+  m[0] = (float)((sxx - (s1x * s1x) / kd) / kd);  // (0,0)
+  m[1] = (float)((sxy - (s1x * s1y) / kd) / kd);  // (1,0)
+  m[2] = (float)((sxz - (s1x * s1z) / kd) / kd);  // (2,0)
+  m[4] = (float)((syy - (s1y * s1y) / kd) / kd);  // (1,1)
+  m[5] = (float)((syz - (s1y * s1z) / kd) / kd);  // (2,1)
+  m[8] = (float)((szz - (s1z * s1z) / kd) / kd);  // (2,2)
+  m[3] = m[6] = m[7] = 0.f;                       // upper triangle: never read
+  float ev[3], V[9];
+  if (!sym_eigen<3>(m, ev, V)) {
+    out[i] = make_float4(qnan, qnan, qnan, qnan);
+    return;
+  }
+  float nx = V[0], ny = V[1], nz = V[2];
+  const float den = (ev[0] + ev[1]) + ev[2];
+  const float curv = den == 0.f ? 0.f : ev[0] / den;
+  if (((vp.x - cx) * (double)nx + (vp.y - cy) * (double)ny) + (vp.z - cz) * (double)nz < 0.0) {
+    nx = -nx;
+    ny = -ny;
+    nz = -nz;
+  }
+  out[i] = make_float4(nx, ny, nz, curv);
+}
+
 // ---- visibility pass: one sweep's sensor pose and range image (include/loam_b200.h "loam_b200_dense_visibility")
 constexpr double DENSE_RAD2DEG = 180.0 / 3.14159265358979323846;
 constexpr unsigned DENSE_NO_RETURN = 0xffffffffu;  // empty pixel (above the bits of +inf, like every float bit pattern
@@ -364,6 +456,7 @@ struct DenseMap {
   DevBuf<int> slots, ints;        // export: slot of each compacted voxel; [0] runs, [1] new voxels, [2] compaction counter
   DevBuf<float4> out;
   DevBuf<unsigned> out_count, out_evidence;
+  DevBuf<float4> normals;         // export with normals: (nx, ny, nz, curvature) per exported voxel
   double vis_h_res = 0.0, vis_v_res = 0.0, vis_margin = 0.0;  // visibility pass (vis_h_res == 0: off)
   int vis_rows = 0, vis_cols = 0;
   DevBuf<unsigned> image;         // range image of the sweep being observed (float bits, DENSE_NO_RETURN when empty)
@@ -387,7 +480,7 @@ struct DenseMap {
     sort.keys_a.release(); sort.keys_b.release(); sort.vals_a.release(); sort.vals_b.release(); sort.hist.release();
     keys64.release(); skeys.release(); pos.release(); rank.release(); run_key.release(); run_count.release();
     run_sum.release(); run_slot.release(); slots.release(); ints.release(); out.release(); out_count.release();
-    out_evidence.release(); image.release();
+    out_evidence.release(); normals.release(); image.release();
     ctr.release(); ctr_host.release();
     if (ev_in) cudaEventDestroy(ev_in);
     if (ev_done) cudaEventDestroy(ev_done);

@@ -130,6 +130,41 @@ void BasicLaserMapping::denseMapFiltered(Cloud& out, double maxMissRatio, std::v
   b200::unpack(buf.data(), (size_t)got, out);
 }
 
+void BasicLaserMapping::denseMapNormals(pcl::PointCloud<pcl::PointXYZINormal>& out, double maxMissRatio, int radius,
+                                        const Vector3& viewpoint, std::vector<uint32_t>* counts) {
+  const double vp[3] = {(double)viewpoint.x(), (double)viewpoint.y(), (double)viewpoint.z()};
+  denseMapNormals(out, maxMissRatio, radius, vp, counts);
+}
+
+void BasicLaserMapping::denseMapNormals(pcl::PointCloud<pcl::PointXYZINormal>& out, double maxMissRatio, int radius,
+                                        const double viewpoint[3], std::vector<uint32_t>* counts) {
+  const int n = (int)denseMapStats().voxels;  // the voxels kept are a subset
+  std::vector<float> buf((size_t)n * 4 + 4), nrm((size_t)n * 4 + 4);
+  if (counts) counts->resize((size_t)n + 1);
+  int got = 0;
+  _gpu->check(loam_b200_dense_export_normals(_gpu->get(), maxMissRatio, radius, viewpoint, buf.data(),
+                                             counts ? counts->data() : nullptr, nrm.data(), n, &got),
+              "loam_b200_dense_export_normals");
+  if (counts) counts->resize((size_t)got);
+  out.points.resize((size_t)got);
+  bool finite = true;
+  for (int i = 0; i < got; i++) {
+    pcl::PointXYZINormal& p = out.points[(size_t)i];
+    p.x = buf[4 * i + 0];
+    p.y = buf[4 * i + 1];
+    p.z = buf[4 * i + 2];
+    p.intensity = buf[4 * i + 3];
+    p.normal_x = nrm[4 * i + 0];
+    p.normal_y = nrm[4 * i + 1];
+    p.normal_z = nrm[4 * i + 2];
+    p.curvature = nrm[4 * i + 3];
+    finite = finite && std::isfinite(p.curvature);  // an undefined normal is NaN in all four fields
+  }
+  out.width = (std::uint32_t)got;
+  out.height = 1;
+  out.is_dense = finite;
+}
+
 long long BasicLaserMapping::denseTableSlots() {
   long long n = 0;
   _gpu->check(loam_b200_debug_dense_table_slots(_gpu->get(), &n), "loam_b200_debug_dense_table_slots");

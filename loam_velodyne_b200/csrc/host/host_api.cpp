@@ -563,6 +563,31 @@ int loam_b200_map_dense_export_filtered(void* h, double max_miss_ratio, float* x
     return 0;
   });
 }
+int loam_b200_map_dense_export_normals(void* h, double max_miss_ratio, int radius, const double* viewpoint,
+                                       float* xyzi, unsigned int* counts, float* normals, int cap, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (!viewpoint) { g_err = "loam_b200_map_dense_export_normals: viewpoint is NULL"; return (int)LOAM_B200_ERR_ARG; }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    std::vector<uint32_t> cnt;
+    pcl::PointCloud<pcl::PointXYZINormal> cloud;
+    m->m.denseMapNormals(cloud, max_miss_ratio, radius, viewpoint, counts ? &cnt : nullptr);
+    const int n = (int)cloud.points.size();
+    *n_out = n;
+    if (n > cap) {
+      g_err = "loam_b200_map_dense_export_normals: output capacity too small";
+      return (int)LOAM_B200_ERR_CAPACITY;
+    }
+    for (int i = 0; i < n; i++) {
+      const pcl::PointXYZINormal& p = cloud.points[(size_t)i];
+      const float a[4] = {p.x, p.y, p.z, p.intensity}, b[4] = {p.normal_x, p.normal_y, p.normal_z, p.curvature};
+      std::memcpy(xyzi + 4 * i, a, sizeof(a));
+      std::memcpy(normals + 4 * i, b, sizeof(b));
+    }
+    if (counts && n > 0) std::memcpy(counts, cnt.data(), (size_t)n * sizeof(uint32_t));
+    return 0;
+  });
+}
 int loam_b200_map_debug_dense_table_slots(void* h, long long* out) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;
   return guarded([&] { *out = ((MapH*)h)->m.denseTableSlots(); return 0; });

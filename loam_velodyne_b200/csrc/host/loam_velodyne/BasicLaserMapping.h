@@ -130,6 +130,15 @@ class BasicLaserMapping {
   void denseMapFiltered(pcl::PointCloud<pcl::PointXYZI>& out, double maxMissRatio,
                         std::vector<uint32_t>* counts = nullptr, std::vector<uint16_t>* hits = nullptr,
                         std::vector<uint16_t>* misses = nullptr);
+  // the voxels of denseMapFiltered(maxMissRatio) with a surface normal and curvature each (include/loam_b200.h
+  // "loam_b200_dense_export_normals"): pcl::NormalEstimation over the exported centroids with a box neighbourhood of
+  // `radius` (1..3) voxels on every axis, normals flipped towards `viewpoint` (map frame; PCL's default, the origin, is
+  // the first sweep's sensor position).  Fewer than 3 neighbours: NaN normal and curvature.  Throws on bad arguments.
+  void denseMapNormals(pcl::PointCloud<pcl::PointXYZINormal>& out, double maxMissRatio, int radius,
+                       const Vector3& viewpoint, std::vector<uint32_t>* counts = nullptr);
+  // the same with the viewpoint in double (x, y, z)
+  void denseMapNormals(pcl::PointCloud<pcl::PointXYZINormal>& out, double maxMissRatio, int radius,
+                       const double viewpoint[3], std::vector<uint32_t>* counts = nullptr);
   /** Test hook (not in the reference): slots of the whole-run map's hash table (0 while the map is off). */
   long long denseTableSlots();
 

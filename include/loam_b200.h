@@ -424,6 +424,71 @@ int loam_b200_dense_export_normals(loam_b200_ctx* ctx, double max_miss_ratio, in
 int loam_b200_debug_dense_table_slots(loam_b200_ctx* ctx, long long* out);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Alignment against the whole-run voxel map (csrc/densemap.cuh, DESIGN.md "Alignment against the whole-run voxel map"):
+ * point-to-plane Gauss-Newton of a cloud against a device-resident target of voxel centroids and normals, for
+ * relocalisation in a map built earlier, drift checks of a mapped pose, or placing another sensor's or session's sweeps
+ * in the same map.  Not on the per-sweep path; the result never feeds back into the mapping stage.
+ *   target_build: the target is the export of loam_b200_dense_export_normals(max_miss_ratio, radius, viewpoint) --
+ *           the same voxels, order and bits -- kept on the device as sorted keys, centroids and normals.  A snapshot:
+ *           later inserts do not change it; the next build or load replaces it; destroying the context frees it.
+ *           *n_out = its voxels.  Arguments as export_normals (LOAM_B200_ERR_ARG); without the map, or on a sharded
+ *           context, LOAM_B200_ERR_STATE.
+ *   target_load: the target from n host entries (a map saved earlier): xyzi float[4] centroids, normals float[4]
+ *           (nx, ny, nz, anything: the export_normals layout); a NaN nx means "no normal".  Works with or without the
+ *           map.  An entry's voxel is dense_key_of(centroid, 1.0f / leaf) (the map's voxel rule); entries are sorted
+ *           by it.  LOAM_B200_ERR_ARG for a leaf that is not finite and > 0, a centroid that is not finite or whose
+ *           voxel is outside the key range, or two entries in one voxel.  Export -> load gives back the built target
+ *           exactly: a centroid (float)(S / count) lies between the smallest and largest of its voxel's points and
+ *           floorf(c * inv) is monotone in c, so an exported centroid's voxel is its own voxel.
+ *   A failed build or load leaves no target.
+ *   align_iterate: one iteration over n points (sensor frame, float[4]; host memory, or device memory when
+ *           on_device != 0) at `pose`, fp32 without FMA, each operation rounded on its own:
+ *             q = pointAssociateToMap(pose, p) with the pose's sin / cos (as loam_b200_map_iterate); a non-finite p
+ *               has no correspondence; v = q's voxel (the target's leaf); v outside the key range: none.
+ *             candidates: the target voxels within search_radius (1..3) of v on every axis with a normal, in ascending
+ *               key order (an offset outside the key range does not exist); d = c - q, d2 = (dx*dx + dy*dy) + dz*dz;
+ *               the first smallest d2 wins and is accepted when d2 < gate, gate = s * s with s = (float)search_radius *
+ *               leaf, both rounded to fp32.  The box contains the ball of radius s around q, so an accepted match is
+ *               the exact nearest centroid with a normal within that distance.
+ *             pd2 = (nx*(qx - cx) + ny*(qy - cy)) + nz*(qz - cz); s = 1 - 0.9f * |pd2| / sqrtf(sqrtf((px*px + py*py)
+ *               + pz*pz)) with the SENSOR-frame p; selected when (double)s > 0.1; coeff = (s*nx, s*ny, s*nz, s*pd2).
+ *             Jacobian row and rhs = -coeff.w of loam_b200_map_iterate.
+ *           ne: the normal equations over the selected rows; n_selected; n_corner_selected = 0.  sum_pd2_sq: the fp32
+ *           sum of pd2^2 over the selected rows.  Sums: per warp of 32 points an fp32 xor butterfly, per CTA of 128
+ *           points the 4 warp sums in warp order, then the CTA partials in double (warp w of the last CTA folds CTAs
+ *           w, w + 4, ...; the 4 results added in warp order), rounded to fp32 once -- run-to-run deterministic.
+ *           Per point (each may be NULL): dbg_match = target index (ascending key order) of the accepted match or -1,
+ *           dbg_coeff = coeff (float[4]; 0 without a match), dbg_sel = 1 when selected.
+ *   align: Gauss-Newton from `initial` with the mapping stage's policy (BasicLaserMapping.cpp:826-922): an iteration
+ *           with fewer than 50 selected rows is skipped; 6x6 solve with eigenvalue threshold 100, the degeneracy
+ *           projection computed on the first iteration that reaches the solve and kept; float pose update, sin / cos
+ *           recomputed from the float angles (loam::Angle); stop when deltaR < 0.05 deg and deltaT < 0.05 cm, or after
+ *           max_iterations (1..100).  One kernel launch and a 32-float readback per iteration.  An empty cloud or an
+ *           empty target runs nothing: the pose comes back unchanged with iterations = 0.  Coarse to fine: call twice
+ *           (search_radius 3, then 1 from the first result).
+ *   No target: LOAM_B200_ERR_STATE.  A bad radius or iteration count, a NULL pointer or a non-finite pose (rot, sin,
+ *   cos or pos): LOAM_B200_ERR_ARG.  Launches count under LOAM_B200_K_DENSE.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  float rot[3];    /* aligned rot_x, rot_y, rot_z */
+  float pos[3];
+  int iterations;  /* iterations executed (0: nothing to align) */
+  int n_selected;  /* selected rows of the last executed iteration, at that iteration's input pose */
+  float rms;       /* sqrt(sum pd2^2 / n_selected) of that iteration (double, rounded once; 0 when none selected) */
+  int degenerate;  /* the solve's degeneracy projection is in effect */
+  int converged;   /* stopped by the deltaR / deltaT thresholds, not by max_iterations */
+} loam_b200_align_result;
+
+int loam_b200_dense_target_build(loam_b200_ctx* ctx, double max_miss_ratio, int radius, const double viewpoint[3],
+                                 int* n_out);
+int loam_b200_dense_target_load(loam_b200_ctx* ctx, float leaf, const float* xyzi, const float* normals, int n);
+int loam_b200_dense_align_iterate(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device,
+                                  const loam_b200_pose* pose, int search_radius, loam_b200_normal_eq* ne,
+                                  float* sum_pd2_sq, int32_t* dbg_match, float* dbg_coeff, int8_t* dbg_sel);
+int loam_b200_dense_align(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device, const loam_b200_pose* initial,
+                          int search_radius, int max_iterations, loam_b200_align_result* out);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice
  * of the corner and surface queries; with a communicator the 32-float partial normal equations are all-reduced
  * (NCCL, sum, fp32) on the context's stream directly behind the kernel, so every rank returns the same totals and

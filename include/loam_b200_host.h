@@ -113,6 +113,16 @@ int loam_b200_map_dense_export_normals(void* h, double max_miss_ratio, int radiu
                                        float* xyzi, unsigned int* counts, float* normals, int cap, int* n_out);
 /* test query: loam_b200_debug_dense_table_slots of the mapping object's context (BasicLaserMapping::denseTableSlots) */
 int loam_b200_map_debug_dense_table_slots(void* h, long long* out);
+/* alignment against the whole-run map (BasicLaserMapping::buildDenseTarget / loadDenseTarget / alignToDenseTarget,
+ * include/loam_b200.h "Alignment against the whole-run voxel map"), same in-flight rule as the exports above.
+ * target_build: *n_out = the target's voxels, viewpoint = 3 doubles.  target_load: n entries of xyzi float[4] and
+ * normals float[4] (nx, ny, nz, curvature).  align: n sensor-frame points, initial6 = twist; twist_out6 = the aligned
+ * twist, stats_out4 = iterations, n_selected, degenerate, converged; *rms_out = the point-to-plane RMS (each out may be
+ * NULL except twist_out6). */
+int loam_b200_map_dense_target_build(void* h, double max_miss_ratio, int radius, const double* viewpoint, int* n_out);
+int loam_b200_map_dense_target_load(void* h, float leaf, const float* xyzi, const float* normals, int n);
+int loam_b200_map_dense_align(void* h, const float* xyzi, int n, const float* initial6, int search_radius,
+                              int max_iterations, float* twist_out6, int* stats_out4, float* rms_out);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank
  * then enables sharding on its mapping object (nccl_id128 = NULL: slice the queries only, no collective) */
 int loam_b200_host_nccl_unique_id(unsigned char* out128);

@@ -61,6 +61,11 @@ class LmResult(C.Structure):
     _fields_ = [("rot", C.c_float * 3), ("pos", C.c_float * 3), ("iterations", C.c_int), ("converged", C.c_int)]
 
 
+class AlignResult(C.Structure):
+    _fields_ = [("rot", C.c_float * 3), ("pos", C.c_float * 3), ("iterations", C.c_int), ("n_selected", C.c_int),
+                ("rms", C.c_float), ("degenerate", C.c_int), ("converged", C.c_int)]
+
+
 class NormalEq(C.Structure):
     _fields_ = [("AtA", C.c_float * 36), ("AtB", C.c_float * 6), ("n_selected", C.c_int),
                 ("n_corner_selected", C.c_int)]
@@ -167,6 +172,12 @@ def lib():
         "loam_b200_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
         "loam_b200_dense_export_normals": (C.c_int, [vp, C.c_double, C.c_int, _D, _F, _U, _F, C.c_int, _I]),
         "loam_b200_debug_dense_table_slots": (C.c_int, [vp, _LL]),
+        "loam_b200_dense_target_build": (C.c_int, [vp, C.c_double, C.c_int, _D, _I]),
+        "loam_b200_dense_target_load": (C.c_int, [vp, C.c_float, _F, _F, C.c_int]),
+        "loam_b200_dense_align_iterate": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int,
+                                                    C.POINTER(NormalEq), _F, _I, _F, _B]),
+        "loam_b200_dense_align": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int, C.c_int,
+                                            C.POINTER(AlignResult)]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -219,6 +230,9 @@ def lib():
         "loam_b200_map_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
         "loam_b200_map_dense_export_normals": (C.c_int, [vp, C.c_double, C.c_int, _D, _F, _U, _F, C.c_int, _I]),
         "loam_b200_map_debug_dense_table_slots": (C.c_int, [vp, _LL]),
+        "loam_b200_map_dense_target_build": (C.c_int, [vp, C.c_double, C.c_int, _D, _I]),
+        "loam_b200_map_dense_target_load": (C.c_int, [vp, C.c_float, _F, _F, C.c_int]),
+        "loam_b200_map_dense_align": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.c_int, _F, _I, _F]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_map_kernel_profile": (C.c_int, [vp, C.c_int, _D]),
@@ -620,6 +634,56 @@ class Ctx:
     def dense_clear(self):
         self._ck(self.L.loam_b200_dense_clear(self.h), "dense_clear")
 
+    # ---- alignment against the whole-run voxel map (include/loam_b200.h "Alignment against the whole-run voxel map")
+    def dense_target_build(self, max_miss_ratio=None, radius=1, viewpoint=(0.0, 0.0, 0.0)):
+        """Snapshot dense_export_normals(max_miss_ratio, radius, viewpoint) on the device as the alignment target ->
+        its voxel count."""
+        ratio = math.inf if max_miss_ratio is None else float(max_miss_ratio)
+        vp = np.ascontiguousarray(viewpoint, np.float64).reshape(3)
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_target_build(self.h, ratio, int(radius), vp.ctypes.data_as(_D), C.byref(n)),
+                 "dense_target_build")
+        return n.value
+
+    def dense_target_load(self, leaf, centroids, normals):
+        """The alignment target from host arrays (N x 4 centroids, N x 4 normals as dense_export_normals returns them;
+        a NaN nx: no normal), e.g. a map saved from an earlier session."""
+        c, nr = _pts(centroids), _pts(normals)
+        if c.shape[0] != nr.shape[0]:
+            raise ValueError("dense_target_load: centroids and normals differ in length")
+        self._ck(self.L.loam_b200_dense_target_load(self.h, np.float32(leaf), _fp(c), _fp(nr), c.shape[0]),
+                 "dense_target_load")
+
+    def dense_align_iterate(self, pts, twist6, search_radius=1, debug=False):
+        """One point-to-plane iteration of sensor-frame pts at twist6 against the target -> (normal equations,
+        sum of pd2^2 over the selected rows); with debug=True also (match N int32, coeff N x 4, selected N int8)."""
+        a = _pts(pts)
+        n = a.shape[0]
+        p = make_pose(twist6)
+        ne = NormalEq()
+        ss = np.zeros(1, np.float32)
+        if debug:
+            match = np.zeros(max(n, 1), np.int32)
+            coeff = np.zeros((max(n, 1), 4), np.float32)
+            sel = np.zeros(max(n, 1), np.int8)
+            self._ck(self.L.loam_b200_dense_align_iterate(self.h, _fp(a), n, 0, C.byref(p), int(search_radius),
+                                                          C.byref(ne), _fp(ss), _ip(match), _fp(coeff),
+                                                          sel.ctypes.data_as(_B)), "dense_align_iterate")
+            return _ne(ne), ss[0], match[:n].copy(), coeff[:n].copy(), sel[:n].copy()
+        self._ck(self.L.loam_b200_dense_align_iterate(self.h, _fp(a), n, 0, C.byref(p), int(search_radius),
+                                                      C.byref(ne), _fp(ss), None, None, None), "dense_align_iterate")
+        return _ne(ne), ss[0]
+
+    def dense_align(self, pts, twist6, search_radius=1, max_iterations=10):
+        """Gauss-Newton of sensor-frame pts against the target from twist6 -> (twist6 float32, {"iterations",
+        "n_selected", "rms", "degenerate", "converged"}).  Coarse to fine: search_radius 3, then 1 from the result."""
+        a = _pts(pts)
+        p = make_pose(twist6)
+        r = AlignResult()
+        self._ck(self.L.loam_b200_dense_align(self.h, _fp(a), a.shape[0], 0, C.byref(p), int(search_radius),
+                                              int(max_iterations), C.byref(r)), "dense_align")
+        return _align_out(list(r.rot) + list(r.pos), r.iterations, r.n_selected, r.rms, r.degenerate, r.converged)
+
     def profile(self, on=True):
         self.L.loam_b200_profile_enable(self.h, 1 if on else 0)
         self.L.loam_b200_profile_reset(self.h)
@@ -673,6 +737,12 @@ def _dense_export_normals(fn, max_miss_ratio, radius, viewpoint, n, ck):
     ck(fn(ratio, int(radius), vp.ctypes.data_as(_D), _fp(pts), cnt.ctypes.data_as(_U), _fp(nrm), n, C.byref(got)))
     k = got.value
     return pts[:k].copy(), cnt[:k].copy(), nrm[:k].copy()
+
+
+def _align_out(twist, iterations, n_selected, rms, degenerate, converged):
+    return np.array(twist, np.float32), {"iterations": int(iterations), "n_selected": int(n_selected),
+                                         "rms": np.float32(rms), "degenerate": bool(degenerate),
+                                         "converged": bool(converged)}
 
 
 def _ne(ne: NormalEq):
@@ -861,6 +931,35 @@ class LaserMapping(_Handle):
         out = C.c_longlong(0)
         self._ck(self.L.loam_b200_map_debug_dense_table_slots(self.h, C.byref(out)), "denseTableSlots")
         return out.value
+
+    def build_dense_target(self, max_miss_ratio=None, radius=1, viewpoint=(0.0, 0.0, 0.0)):
+        """BasicLaserMapping::buildDenseTarget: snapshot dense_map_normals(...) as the alignment target -> voxels."""
+        ratio = math.inf if max_miss_ratio is None else float(max_miss_ratio)
+        vp = np.ascontiguousarray(viewpoint, np.float64).reshape(3)
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_map_dense_target_build(self.h, ratio, int(radius), vp.ctypes.data_as(_D),
+                                                         C.byref(n)), "buildDenseTarget")
+        return n.value
+
+    def load_dense_target(self, leaf, centroids, normals):
+        """BasicLaserMapping::loadDenseTarget from host arrays; see Ctx.dense_target_load."""
+        c, nr = _pts(centroids), _pts(normals)
+        if c.shape[0] != nr.shape[0]:
+            raise ValueError("load_dense_target: centroids and normals differ in length")
+        self._ck(self.L.loam_b200_map_dense_target_load(self.h, np.float32(leaf), _fp(c), _fp(nr), c.shape[0]),
+                 "loadDenseTarget")
+
+    def align_to_dense_target(self, pts, twist6, search_radius=1, max_iterations=10):
+        """BasicLaserMapping::alignToDenseTarget; returns what Ctx.dense_align returns."""
+        a = _pts(pts)
+        t = np.ascontiguousarray(twist6, np.float32).reshape(6)
+        out = np.zeros(6, np.float32)
+        st = np.zeros(4, np.int32)
+        rms = np.zeros(1, np.float32)
+        self._ck(self.L.loam_b200_map_dense_align(self.h, _fp(a), a.shape[0], _fp(t), int(search_radius),
+                                                  int(max_iterations), _fp(out), _ip(st), _fp(rms)),
+                 "alignToDenseTarget")
+        return _align_out(out, st[0], st[1], rms[0], st[2], st[3])
 
     def enable_dense_visibility(self, h_res_deg, v_res_deg, margin):
         """Count, per voxel of the whole-run map, the mapped sweeps that see through it (h_res_deg = 0: off); filter

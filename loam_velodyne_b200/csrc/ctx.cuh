@@ -185,6 +185,7 @@ struct SortScratch {
 };
 
 struct DenseMap;  // whole-run voxel map (densemap.cuh), created by loam_b200_dense_enable
+struct DenseTarget;  // registration target of loam_b200_dense_align (densemap.cuh)
 
 }  // namespace loamb
 
@@ -372,6 +373,8 @@ struct loam_b200_ctx {
 
   // whole-run voxel map: null until enabled, so a context without it allocates and launches nothing for it
   loamb::DenseMap* dense = nullptr;
+  // its registration target: null until the first loam_b200_dense_target_build / _load succeeds
+  loamb::DenseTarget* target = nullptr;
 };
 
 namespace loamb {

@@ -22,6 +22,7 @@
 #pragma once
 
 #include "linalg.cuh"
+#include "mapping_lm.cuh"
 #include "voxel.cuh"
 
 namespace loamb {
@@ -367,6 +368,110 @@ dense_normals_kernel(const unsigned long long* __restrict__ skey, const float4* 
   out[i] = make_float4(nx, ny, nz, curv);
 }
 
+// ---- registration target (include/loam_b200.h "loam_b200_dense_target_build" / "_load" / "_align_iterate")
+// load: one thread per sorted entry -- gather key, centroid and normal in key order; flag a key outside the range
+// (DENSE_EMPTY sorts last) with bit 0 and a key equal to its predecessor's with bit 1
+__global__ void dense_target_gather_kernel(const unsigned long long* __restrict__ keys64, const int* __restrict__ order,
+                                           int n, const float4* __restrict__ cent_in, const float4* __restrict__ nrm_in,
+                                           unsigned long long* __restrict__ skey, float4* __restrict__ cent,
+                                           float4* __restrict__ nrm, int* __restrict__ bad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int o = order[i];
+  const unsigned long long k = keys64[o];
+  skey[i] = k;
+  cent[i] = cent_in[o];
+  nrm[i] = nrm_in[o];
+  if (k == DENSE_EMPTY) atomicOr(bad, 1);
+  else if (i > 0 && keys64[order[i - 1]] == k) atomicOr(bad, 2);
+}
+
+// One Gauss-Newton iteration of a cloud against the target, one thread per point (point i in CTA i / LM_THREADS):
+//   q = associate_to_map(pose, p); v = voxel of q (dense_key_of with the target's leaf);
+//   candidates: the target voxels within `radius` of v on every axis whose normal_x is not NaN, visited in ascending key
+//   order by the row walk of dense_normals_kernel (rows outside the key range are skipped and never wrap); the first
+//   smallest d2 = (dx*dx + dy*dy) + dz*dz, d = c - q, wins when d2 < gate;
+//   pd2 = (nx*(qx - cx) + ny*(qy - cy)) + nz*(qz - cz); s = 1 - 0.9f*|pd2| / sqrtf(sqrtf(|p|^2)) with the SENSOR-frame p;
+//   selected when (double)s > 0.1; coeff = s * (n, pd2); Jacobian row and rhs of the scan-to-map kernels.
+// Slots 0..26 of the 32 sums: AtA (upper triangle) and AtB; 27: selected rows; 28: sum of pd2^2 over them.  The
+// reduction is reduce_normal_equations (fp32 xor butterfly per warp, the 4 warp sums in warp order, CTA partials folded
+// in double in fixed order).  The library is built without FMA contraction, as tests/align_reference.py assumes.
+__global__ void __launch_bounds__(LM_THREADS)
+dense_align_kernel(const unsigned long long* __restrict__ skey, const float4* __restrict__ cent,
+                   const float4* __restrict__ nrm, int m, float inv, int radius, float gate,
+                   const float4* __restrict__ pts, int n, MapIterArgs a, float* __restrict__ partials,
+                   float* __restrict__ result, unsigned int* ticket, int* __restrict__ dbg_match,
+                   float4* __restrict__ dbg_coeff, int8_t* __restrict__ dbg_sel) {
+  float acc[29];
+#pragma unroll
+  for (int k = 0; k < 29; k++) acc[k] = 0.f;
+  const int i = blockIdx.x * LM_THREADS + threadIdx.x;
+  if (i < n) {  // every thread takes part in the reduction below
+    const float4 po = pts[i];
+    int best = -1;
+    float4 coeff = make_float4(0.f, 0.f, 0.f, 0.f);
+    bool sel = false;
+    if (isfinite(po.x) && isfinite(po.y) && isfinite(po.z)) {
+      float qx, qy, qz;
+      associate_to_map(a, po, qx, qy, qz);
+      const unsigned long long key = dense_key_of(make_float4(qx, qy, qz, 0.f), inv);
+      if (key != DENSE_EMPTY) {
+        const int vx = (int)(key & DENSE_AXIS_MASK), vy = (int)((key >> 21) & DENSE_AXIS_MASK), vz = (int)(key >> 42);
+        const unsigned long long x0 = (unsigned long long)max(vx - radius, 0);
+        const unsigned long long x1 = (unsigned long long)min(vx + radius, DENSE_AXIS - 1);
+        float best_d2 = gate;  // strict < from the gate: the first smallest d2 below it
+        int lo = 0;            // rows ascend in key order: each row's search starts where the previous row ended
+        for (int z = vz - radius; z <= vz + radius; z++) {
+          if (z < 0 || z >= DENSE_AXIS) continue;
+          for (int y = vy - radius; y <= vy + radius; y++) {
+            if (y < 0 || y >= DENSE_AXIS) continue;
+            const unsigned long long row = ((unsigned long long)z << 42) | ((unsigned long long)y << 21);
+            const unsigned long long last = row | x1;
+            int j = dense_lower_bound(skey, lo, m, row | x0);
+            for (; j < m && skey[j] <= last; j++) {
+              if (isnan(nrm[j].x)) continue;
+              const float4 c = cent[j];
+              const float dx = c.x - qx, dy = c.y - qy, dz = c.z - qz;
+              const float d2 = (dx * dx + dy * dy) + dz * dz;
+              if (d2 < best_d2) {
+                best_d2 = d2;
+                best = j;
+              }
+            }
+            lo = j;
+          }
+        }
+      }
+      if (best >= 0) {
+        const float4 c = cent[best], nv = nrm[best];
+        const float pd2 = (nv.x * (qx - c.x) + nv.y * (qy - c.y)) + nv.z * (qz - c.z);
+        const float s = 1.f - 0.9f * fabsf(pd2) / sqrtf(sqrtf(po.x * po.x + po.y * po.y + po.z * po.z));
+        coeff = make_float4(s * nv.x, s * nv.y, s * nv.z, s * pd2);
+        sel = (double)s > 0.1;
+        if (sel) {
+          float row[6], rhs;
+          map_jacobian_row(a, po, coeff, row, rhs);
+          int k = 0;
+#pragma unroll
+          for (int r = 0; r < 6; r++)
+#pragma unroll
+            for (int t = r; t < 6; t++) acc[k++] = row[r] * row[t];
+#pragma unroll
+          for (int r = 0; r < 6; r++) acc[21 + r] = row[r] * rhs;
+          acc[27] = 1.f;
+          acc[28] = pd2 * pd2;
+        }
+      }
+    }
+    if (dbg_match) {
+      dbg_match[i] = best;
+      dbg_coeff[i] = coeff;
+      dbg_sel[i] = sel ? 1 : 0;
+    }
+  }
+  reduce_normal_equations(acc, partials, result, ticket, ResultMailbox{nullptr, 0}, gridDim.x);
+}
+
 // ---- visibility pass: one sweep's sensor pose and range image (include/loam_b200.h "loam_b200_dense_visibility")
 constexpr double DENSE_RAD2DEG = 180.0 / 3.14159265358979323846;
 constexpr unsigned DENSE_NO_RETURN = 0xffffffffu;  // empty pixel (above the bits of +inf, like every float bit pattern
@@ -486,6 +591,30 @@ struct DenseMap {
     if (ev_done) cudaEventDestroy(ev_done);
     if (ev_observed) cudaEventDestroy(ev_observed);
     ev_in = ev_done = ev_observed = nullptr;
+  }
+};
+
+// Registration target of loam_b200_dense_align (loam_b200_ctx::target): a snapshot of sorted keys, centroids and
+// normals, built from the map's export or loaded from the host.  Independent of DenseMap, so a context without the map
+// can load one.  The iteration's scratch lives beside it and is used on the context's own stream.
+struct DenseTarget {
+  bool ready = false;             // false until a build or load succeeds (a failed one leaves no target)
+  float leaf = 0.f;
+  int n = 0;
+  DevBuf<unsigned long long> keys, keys64;  // sorted keys; load: the entries' keys in input order
+  DevBuf<float4> cent, nrm;
+  DevBuf<float4> pts;             // the cloud being aligned (a host cloud is uploaded here)
+  DevBuf<float> partials, result; // per-CTA partial sums, the 32 folded sums
+  DevBuf<unsigned> ticket;        // zero between launches (reduce_normal_equations resets it)
+  DevBuf<int> match, flag;
+  DevBuf<float4> coeff;
+  DevBuf<int8_t> sel;
+
+  void release() {
+    keys.release(); keys64.release(); cent.release(); nrm.release(); pts.release(); partials.release();
+    result.release(); ticket.release(); match.release(); flag.release(); coeff.release(); sel.release();
+    n = 0;
+    ready = false;
   }
 };
 

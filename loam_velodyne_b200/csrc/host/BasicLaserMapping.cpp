@@ -7,6 +7,7 @@
 
 #include <chrono>
 #include <cmath>
+#include <cstring>
 
 #include "b200_runtime.h"
 #include "host_math.h"
@@ -163,6 +164,55 @@ void BasicLaserMapping::denseMapNormals(pcl::PointCloud<pcl::PointXYZINormal>& o
   out.width = (std::uint32_t)got;
   out.height = 1;
   out.is_dense = finite;
+}
+
+size_t BasicLaserMapping::buildDenseTarget(double maxMissRatio, int radius, const Vector3& viewpoint) {
+  const double vp[3] = {(double)viewpoint.x(), (double)viewpoint.y(), (double)viewpoint.z()};
+  return buildDenseTarget(maxMissRatio, radius, vp);
+}
+
+size_t BasicLaserMapping::buildDenseTarget(double maxMissRatio, int radius, const double viewpoint[3]) {
+  int n = 0;
+  _gpu->check(loam_b200_dense_target_build(_gpu->get(), maxMissRatio, radius, viewpoint, &n),
+              "loam_b200_dense_target_build");
+  return (size_t)n;
+}
+
+void BasicLaserMapping::loadDenseTarget(float leaf, const pcl::PointCloud<pcl::PointXYZINormal>& target) {
+  const size_t n = target.points.size();
+  std::vector<float> xyzi(n * 4 + 4), nrm(n * 4 + 4);
+  for (size_t i = 0; i < n; i++) {
+    const pcl::PointXYZINormal& p = target.points[i];
+    const float a[4] = {p.x, p.y, p.z, p.intensity}, b[4] = {p.normal_x, p.normal_y, p.normal_z, p.curvature};
+    std::memcpy(&xyzi[4 * i], a, sizeof(a));
+    std::memcpy(&nrm[4 * i], b, sizeof(b));
+  }
+  _gpu->check(loam_b200_dense_target_load(_gpu->get(), leaf, xyzi.data(), nrm.data(), (int)n),
+              "loam_b200_dense_target_load");
+}
+
+BasicLaserMapping::DenseAlignResult BasicLaserMapping::alignToDenseTarget(const Cloud& cloud, const Twist& initial,
+                                                                          int searchRadius, int maxIterations) {
+  b200::pack(cloud, _bufA);
+  loam_b200_pose pose;
+  b200::fillPose(initial, pose);
+  loam_b200_align_result res;
+  _gpu->check(loam_b200_dense_align(_gpu->get(), _bufA.data(), (int)cloud.points.size(), 0, &pose, searchRadius,
+                                    maxIterations, &res),
+              "loam_b200_dense_align");
+  DenseAlignResult out;
+  out.pose.rot_x = res.rot[0];
+  out.pose.rot_y = res.rot[1];
+  out.pose.rot_z = res.rot[2];
+  out.pose.pos.x() = res.pos[0];
+  out.pose.pos.y() = res.pos[1];
+  out.pose.pos.z() = res.pos[2];
+  out.iterations = (size_t)res.iterations;
+  out.nSelected = (size_t)res.n_selected;
+  out.rms = res.rms;
+  out.degenerate = res.degenerate != 0;
+  out.converged = res.converged != 0;
+  return out;
 }
 
 long long BasicLaserMapping::denseTableSlots() {

@@ -588,6 +588,62 @@ int loam_b200_map_dense_export_normals(void* h, double max_miss_ratio, int radiu
     return 0;
   });
 }
+int loam_b200_map_dense_target_build(void* h, double max_miss_ratio, int radius, const double* viewpoint, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (!viewpoint || !n_out) { g_err = "loam_b200_map_dense_target_build: NULL argument"; return (int)LOAM_B200_ERR_ARG; }
+  return guarded([&] {
+    *n_out = (int)((MapH*)h)->m.buildDenseTarget(max_miss_ratio, radius, viewpoint);
+    return 0;
+  });
+}
+int loam_b200_map_dense_target_load(void* h, float leaf, const float* xyzi, const float* normals, int n) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && (!xyzi || !normals))) {
+    g_err = "loam_b200_map_dense_target_load: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    pcl::PointCloud<pcl::PointXYZINormal> target;
+    target.points.resize((size_t)n);
+    for (int i = 0; i < n; i++) {
+      pcl::PointXYZINormal& p = target.points[(size_t)i];
+      p.x = xyzi[4 * i + 0]; p.y = xyzi[4 * i + 1]; p.z = xyzi[4 * i + 2]; p.intensity = xyzi[4 * i + 3];
+      p.normal_x = normals[4 * i + 0]; p.normal_y = normals[4 * i + 1]; p.normal_z = normals[4 * i + 2];
+      p.curvature = normals[4 * i + 3];
+    }
+    ((MapH*)h)->m.loadDenseTarget(leaf, target);
+    return 0;
+  });
+}
+int loam_b200_map_dense_align(void* h, const float* xyzi, int n, const float* initial6, int search_radius,
+                              int max_iterations, float* twist_out6, int* stats_out4, float* rms_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && !xyzi) || !initial6 || !twist_out6) {
+    g_err = "loam_b200_map_dense_align: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, xyzi, n);
+    loam::Twist initial;
+    initial.rot_x = initial6[0];
+    initial.rot_y = initial6[1];
+    initial.rot_z = initial6[2];
+    initial.pos.x() = initial6[3];
+    initial.pos.y() = initial6[4];
+    initial.pos.z() = initial6[5];
+    const auto r = m->m.alignToDenseTarget(m->scratchA, initial, search_radius, max_iterations);
+    twist6(r.pose, twist_out6);
+    if (stats_out4) {
+      stats_out4[0] = (int)r.iterations;
+      stats_out4[1] = (int)r.nSelected;
+      stats_out4[2] = r.degenerate ? 1 : 0;
+      stats_out4[3] = r.converged ? 1 : 0;
+    }
+    if (rms_out) *rms_out = r.rms;
+    return 0;
+  });
+}
 int loam_b200_map_debug_dense_table_slots(void* h, long long* out) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;
   return guarded([&] { *out = ((MapH*)h)->m.denseTableSlots(); return 0; });

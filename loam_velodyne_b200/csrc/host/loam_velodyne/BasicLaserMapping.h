@@ -141,6 +141,27 @@ class BasicLaserMapping {
                        const double viewpoint[3], std::vector<uint32_t>* counts = nullptr);
   /** Test hook (not in the reference): slots of the whole-run map's hash table (0 while the map is off). */
   long long denseTableSlots();
+  // Alignment against the whole-run map (include/loam_b200.h "Alignment against the whole-run voxel map"): point-to-plane
+  // Gauss-Newton of a sensor-frame cloud against a target of voxel centroids and normals on the GPU -- relocalisation
+  // in a map built earlier, drift checks of a mapped pose, another sensor's or session's sweeps in the same map.
+  // buildDenseTarget snapshots denseMapNormals(maxMissRatio, radius, viewpoint) as the target and returns its voxel
+  // count; loadDenseTarget takes one from a saved cloud (a NaN normal_x: no normal; throws on entries outside the key
+  // range or two in one voxel).  alignToDenseTarget runs the mapping stage's loop (skip below 50 correspondences,
+  // eigenvalue threshold 100, deltaR 0.05 deg / deltaT 0.05 cm) from `initial`; refine coarse to fine by calling it
+  // with searchRadius 3, then 1 from the first result.  The result never changes this object's poses or maps.
+  struct DenseAlignResult {
+    Twist pose;
+    size_t iterations;  // executed (0: empty cloud or empty target)
+    size_t nSelected;   // correspondences of the last executed iteration, at its input pose
+    float rms;          // their point-to-plane RMS (metres)
+    bool degenerate;    // the degeneracy projection was in effect
+    bool converged;     // stopped by the thresholds, not by maxIterations
+  };
+  size_t buildDenseTarget(double maxMissRatio, int radius, const Vector3& viewpoint);
+  size_t buildDenseTarget(double maxMissRatio, int radius, const double viewpoint[3]);
+  void loadDenseTarget(float leaf, const pcl::PointCloud<pcl::PointXYZINormal>& target);
+  DenseAlignResult alignToDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& cloud, const Twist& initial,
+                                      int searchRadius, int maxIterations);
 
  private:
   typedef pcl::PointCloud<pcl::PointXYZI> Cloud;

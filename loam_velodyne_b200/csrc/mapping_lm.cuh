@@ -169,6 +169,23 @@ __device__ __forceinline__ void associate_to_map(const MapIterArgs& a, const flo
   z = z3 + a.tz;
 }
 
+// Jacobian row of a selected correspondence with coefficient `coeff` at sensor-frame point po, and its right-hand side
+// (BasicLaserMapping.cpp:842-861); shared by the scan-to-map kernels and the whole-run map alignment (densemap.cuh)
+__device__ __forceinline__ void map_jacobian_row(const MapIterArgs& a, const float4& po, const float4& coeff,
+                                                 float row[6], float& rhs) {
+  row[0] = (a.A[0] * po.x + a.A[1] * po.y + a.A[2] * po.z) * coeff.x +
+           (a.A[3] * po.x + a.A[4] * po.y + a.A[5] * po.z) * coeff.y +
+           (a.A[6] * po.x + a.A[7] * po.y + a.A[8] * po.z) * coeff.z;
+  row[1] = (a.B[0] * po.x + a.B[1] * po.y + a.B[2] * po.z) * coeff.x +
+           (a.B[6] * po.x + a.B[7] * po.y + a.B[8] * po.z) * coeff.z;
+  row[2] = (a.C[0] * po.x + a.C[1] * po.y) * coeff.x + (a.C[3] * po.x + a.C[4] * po.y) * coeff.y +
+           (a.C[6] * po.x + a.C[7] * po.y) * coeff.z;
+  row[3] = coeff.x;
+  row[4] = coeff.y;
+  row[5] = coeff.z;
+  rhs = -coeff.w;
+}
+
 // stack points: pointAssociateToMap with the predicted pose then pointAssociateTobeMapped back into the sensor frame
 // (BasicLaserMapping.cpp:282-292 and :512-516; the round trip is not an identity in fp32 and is reproduced).
 // Negated angles flip the sine only (Angle.h:47-53).
@@ -533,19 +550,7 @@ map_iterate_kernel(LOOKUP corner_grid, LOOKUP surf_grid, const float4* queries, 
         dbg_coeff[qi] = coeff;
         dbg_sel[qi] = sel ? 1 : 0;
       }
-      if (sel) {
-        row[0] = (a.A[0] * po.x + a.A[1] * po.y + a.A[2] * po.z) * coeff.x +
-                 (a.A[3] * po.x + a.A[4] * po.y + a.A[5] * po.z) * coeff.y +
-                 (a.A[6] * po.x + a.A[7] * po.y + a.A[8] * po.z) * coeff.z;
-        row[1] = (a.B[0] * po.x + a.B[1] * po.y + a.B[2] * po.z) * coeff.x +
-                 (a.B[6] * po.x + a.B[7] * po.y + a.B[8] * po.z) * coeff.z;
-        row[2] = (a.C[0] * po.x + a.C[1] * po.y) * coeff.x + (a.C[3] * po.x + a.C[4] * po.y) * coeff.y +
-                 (a.C[6] * po.x + a.C[7] * po.y) * coeff.z;
-        row[3] = coeff.x;
-        row[4] = coeff.y;
-        row[5] = coeff.z;
-        rhs = -coeff.w;
-      }
+      if (sel) map_jacobian_row(a, po, coeff, row, rhs);
     }
     // 21 + 6 + 2 sums over the warp; after the xor butterfly every lane holds every sum, lane k keeps sum k
     float mine = 0.f;
@@ -727,19 +732,7 @@ map_iterate_v2_kernel(LOOKUP corner_grid, LOOKUP surf_grid, const float4* querie
           dbg_coeff[qi] = coeff;
           dbg_sel[qi] = sel ? 1 : 0;
         }
-        if (sel) {
-          row[0] = (a.A[0] * po.x + a.A[1] * po.y + a.A[2] * po.z) * coeff.x +
-                   (a.A[3] * po.x + a.A[4] * po.y + a.A[5] * po.z) * coeff.y +
-                   (a.A[6] * po.x + a.A[7] * po.y + a.A[8] * po.z) * coeff.z;
-          row[1] = (a.B[0] * po.x + a.B[1] * po.y + a.B[2] * po.z) * coeff.x +
-                   (a.B[6] * po.x + a.B[7] * po.y + a.B[8] * po.z) * coeff.z;
-          row[2] = (a.C[0] * po.x + a.C[1] * po.y) * coeff.x + (a.C[3] * po.x + a.C[4] * po.y) * coeff.y +
-                   (a.C[6] * po.x + a.C[7] * po.y) * coeff.z;
-          row[3] = coeff.x;
-          row[4] = coeff.y;
-          row[5] = coeff.z;
-          rhs = -coeff.w;
-        }
+        if (sel) map_jacobian_row(a, po, coeff, row, rhs);
       }
       if (b + 2 * (int)gridDim.x < n_blocks) named_bar_arrive(BAR_EMPTY + half, MAPV2_THREADS);  // this half may be refilled
       float mine = 0.f;

@@ -489,6 +489,84 @@ int loam_b200_dense_align(loam_b200_ctx* ctx, const float* xyzi, int n, int on_d
                           int search_radius, int max_iterations, loam_b200_align_result* out);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Relocalisation against the whole-run voxel map (DESIGN.md "Relocalisation against the whole-run voxel map"): one
+ * cloud at many poses against the target above, for a restart or a tracking loss where the position is roughly known
+ * (the last saved pose, GNSS) and the heading is not.  Not on the per-sweep path; the result never feeds back into
+ * the mapping stage.  The target, cloud, radius, iteration and error rules are those of align_iterate / align.
+ *   dense_score: the k poses (1 <= k <= 1 << 20) in one upload of the cloud and one launch per chunk of at most
+ *           65535 poses -> per pose exactly what align_iterate returns at that pose in ne.n_selected and sum_pd2_sq.
+ *   dense_align_batch: k independent runs of align from initial[h] -> out[h], equal to dense_align from initial[h]
+ *           bit for bit (the same host solve and degeneracy projection per run).  Per iteration one launch per chunk
+ *           over the runs still going and one readback; a run leaves when it converges or after max_iterations.
+ *           dense_align is this with k = 1.
+ *   reloc_grid: host only.  The LOAM frame has y up: heading is rot_y, the ground plane x-z.  The poses, j outer,
+ *           then iz, then ix, each ascending from -steps to +steps:
+ *             rot_y = prior.rot_y + (float)((double)j * yaw_step_deg * pi / 180), rot_x / rot_z the prior's,
+ *             pos = (prior.x + (float)ix * xz_step, prior.y, prior.z + (float)iz * xz_step), all in float;
+ *             sin_ / cos_ = std::sin / std::cos of the float angles (loam::Angle).
+ *           (2 yaw_steps + 1) (2 xz_steps + 1)^2 poses, at most 1 << 20; a full circle is yaw_steps =
+ *           ceil(180 / yaw_step_deg) (the duplicated +-180 deg is harmless).  *n_out = that count;
+ *           LOAM_B200_ERR_CAPACITY when it exceeds cap.  LOAM_B200_ERR_ARG for a step that is not finite and > 0, a
+ *           negative step count, a non-finite prior or a NULL pointer.
+ *   dense_relocalize: built on the two calls above, in this order:
+ *           1. score every hypothesis at score_radius;
+ *           2. keep the `keep` best (1..1024) by selected descending, then index ascending; one with fewer than 50
+ *              selected is never kept (it could not take a step);
+ *           3. dense_align_batch of the kept poses at coarse_radius, then at fine_radius from those results (sin /
+ *              cos recomputed from the float angles), each with max_iterations;
+ *           4. score at fine_radius at the refined poses -> selected, rms = sqrt(sum pd2^2 / selected) in double,
+ *              rounded once (0 when none);
+ *           5. rank by selected descending, then rms ascending, then keep order;
+ *           6. drop a candidate whose translation differs from a better-ranked survivor's by less than dedup_m AND
+ *              whose rotation differs by less than dedup_deg (the angle of R(a)^T R(b), in double);
+ *           7. write the first cap survivors; *n_out = candidates written (0, with no error, when nothing reaches 50).
+ *           The gap between candidates 0 and 1 is the ambiguity of the result.  A host cloud is uploaded once.
+ *   Errors: no target LOAM_B200_ERR_STATE; a bad radius, iteration count, keep, k, cap or dedup threshold (negative
+ *   or not finite), a NULL pointer or a non-finite pose LOAM_B200_ERR_ARG.  An empty cloud or target runs nothing:
+ *   scores are 0, every run returns its initial pose with iterations = 0, relocalize returns no candidate.
+ *   Launches count under LOAM_B200_K_DENSE.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int score_radius;   /* search radius of the first score (1..3) */
+  int coarse_radius;  /* of the first refinement */
+  int fine_radius;    /* of the second refinement and the final score */
+  int keep;           /* hypotheses refined (1..1024) */
+  int max_iterations; /* per refinement (1..100) */
+  float dedup_m;      /* duplicate: closer than this in translation (>= 0) ... */
+  float dedup_deg;    /* ... and than this in rotation (>= 0) */
+} loam_b200_reloc_params;
+
+typedef struct {
+  int hypothesis;                /* index into the hypotheses given */
+  int score_selected;            /* its selected count in the first score */
+  loam_b200_align_result coarse; /* the refinement at coarse_radius */
+  loam_b200_align_result fine;   /* the refinement at fine_radius from the coarse pose: the candidate's pose */
+  int selected;                  /* the final score at the fine pose */
+  float rms;
+} loam_b200_reloc_candidate;
+
+/* Recommended parameters, chosen from the measured basin (DESIGN.md "Relocalisation against the whole-run voxel
+ * map"): a full-circle yaw grid at 2 deg (90 steps to each side) and an x-z grid of 0.4 m steps four to each side of
+ * the prior (+-1.6 m), 181 x 81 = 14661 poses.  The nearest grid pose is then within 1 deg and 0.2 m per axis (0.28 m)
+ * of the truth, a corner from which every measured coarse-to-fine run converged (VLP-16 and HDL-64E, leaf 0.1 and 0.2,
+ * 8 directions, both yaw signs). */
+#define LOAM_B200_RELOC_YAW_STEP_DEG 2.0f
+#define LOAM_B200_RELOC_XZ_STEP 0.4f
+#define LOAM_B200_RELOC_XZ_STEPS 4
+#define LOAM_B200_RELOC_PARAMS_DEFAULT {3, 3, 1, 16, 30, 0.5f, 5.0f}
+
+int loam_b200_dense_score(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device, const loam_b200_pose* poses,
+                          int k, int search_radius, int32_t* n_selected, float* sum_pd2_sq);
+int loam_b200_dense_align_batch(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device,
+                                const loam_b200_pose* initial, int k, int search_radius, int max_iterations,
+                                loam_b200_align_result* out);
+int loam_b200_reloc_grid(const loam_b200_pose* prior, float yaw_step_deg, int yaw_steps, float xz_step, int xz_steps,
+                         loam_b200_pose* out, int cap, int* n_out);
+int loam_b200_dense_relocalize(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device,
+                               const loam_b200_pose* hyps, int k, const loam_b200_reloc_params* prm,
+                               loam_b200_reloc_candidate* out, int cap, int* n_out);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice
  * of the corner and surface queries; with a communicator the 32-float partial normal equations are all-reduced
  * (NCCL, sum, fp32) on the context's stream directly behind the kernel, so every rank returns the same totals and

@@ -11,6 +11,8 @@
 #ifndef LOAM_B200_HOST_H
 #define LOAM_B200_HOST_H
 
+#include "loam_b200.h"
+
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -123,6 +125,18 @@ int loam_b200_map_dense_target_build(void* h, double max_miss_ratio, int radius,
 int loam_b200_map_dense_target_load(void* h, float leaf, const float* xyzi, const float* normals, int n);
 int loam_b200_map_dense_align(void* h, const float* xyzi, int n, const float* initial6, int search_radius,
                               int max_iterations, float* twist_out6, int* stats_out4, float* rms_out);
+/* relocalisation against that target (BasicLaserMapping::scoreDenseTarget / alignToDenseTarget over a vector /
+ * relocalizeInDenseTarget, include/loam_b200.h "Relocalisation against the whole-run voxel map"), same in-flight rule.
+ * k twists of 6 floats each.  score: n_selected[k], sum_pd2_sq[k].  align_batch: per run h, twist_out6[6h..],
+ * stats_out4[4h..] and rms_out[h] as align (stats_out4 and rms_out may be NULL).  relocalize: at most cap candidates
+ * into out, *n_out = candidates written. */
+int loam_b200_map_dense_score(void* h, const float* xyzi, int n, const float* poses6, int k, int search_radius,
+                              int* n_selected, float* sum_pd2_sq);
+int loam_b200_map_dense_align_batch(void* h, const float* xyzi, int n, const float* initial6, int k, int search_radius,
+                                    int max_iterations, float* twist_out6, int* stats_out4, float* rms_out);
+int loam_b200_map_dense_relocalize(void* h, const float* xyzi, int n, const float* hyps6, int k,
+                                   const loam_b200_reloc_params* prm, loam_b200_reloc_candidate* out, int cap,
+                                   int* n_out);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank
  * then enables sharding on its mapping object (nccl_id128 = NULL: slice the queries only, no collective) */
 int loam_b200_host_nccl_unique_id(unsigned char* out128);

@@ -66,6 +66,25 @@ class AlignResult(C.Structure):
                 ("rms", C.c_float), ("degenerate", C.c_int), ("converged", C.c_int)]
 
 
+class RelocParams(C.Structure):
+    """loam_b200_reloc_params; default(): the recommended parameters (LOAM_B200_RELOC_PARAMS_DEFAULT)."""
+    _fields_ = [("score_radius", C.c_int), ("coarse_radius", C.c_int), ("fine_radius", C.c_int), ("keep", C.c_int),
+                ("max_iterations", C.c_int), ("dedup_m", C.c_float), ("dedup_deg", C.c_float)]
+
+    @staticmethod
+    def default():
+        return RelocParams(3, 3, 1, 16, 30, np.float32(0.5), np.float32(5.0))
+
+
+class RelocCandidate(C.Structure):
+    _fields_ = [("hypothesis", C.c_int), ("score_selected", C.c_int), ("coarse", AlignResult), ("fine", AlignResult),
+                ("selected", C.c_int), ("rms", C.c_float)]
+
+
+# recommended relocalisation grid (include/loam_b200.h): full circle at 2 deg, 0.4 m steps four to each side of the prior
+RELOC_YAW_STEP_DEG, RELOC_XZ_STEP, RELOC_XZ_STEPS = 2.0, 0.4, 4
+
+
 class NormalEq(C.Structure):
     _fields_ = [("AtA", C.c_float * 36), ("AtB", C.c_float * 6), ("n_selected", C.c_int),
                 ("n_corner_selected", C.c_int)]
@@ -178,6 +197,13 @@ def lib():
                                                     C.POINTER(NormalEq), _F, _I, _F, _B]),
         "loam_b200_dense_align": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int, C.c_int,
                                             C.POINTER(AlignResult)]),
+        "loam_b200_dense_score": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int, C.c_int, _I, _F]),
+        "loam_b200_dense_align_batch": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int, C.c_int, C.c_int,
+                                                  C.POINTER(AlignResult)]),
+        "loam_b200_reloc_grid": (C.c_int, [C.POINTER(Pose), C.c_float, C.c_int, C.c_float, C.c_int, C.POINTER(Pose),
+                                           C.c_int, _I]),
+        "loam_b200_dense_relocalize": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int,
+                                                 C.POINTER(RelocParams), C.POINTER(RelocCandidate), C.c_int, _I]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -233,6 +259,10 @@ def lib():
         "loam_b200_map_dense_target_build": (C.c_int, [vp, C.c_double, C.c_int, _D, _I]),
         "loam_b200_map_dense_target_load": (C.c_int, [vp, C.c_float, _F, _F, C.c_int]),
         "loam_b200_map_dense_align": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.c_int, _F, _I, _F]),
+        "loam_b200_map_dense_score": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.c_int, _I, _F]),
+        "loam_b200_map_dense_align_batch": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.c_int, C.c_int, _F, _I, _F]),
+        "loam_b200_map_dense_relocalize": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.POINTER(RelocParams),
+                                                     C.POINTER(RelocCandidate), C.c_int, _I]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_map_kernel_profile": (C.c_int, [vp, C.c_int, _D]),
@@ -684,6 +714,42 @@ class Ctx:
                                               int(max_iterations), C.byref(r)), "dense_align")
         return _align_out(list(r.rot) + list(r.pos), r.iterations, r.n_selected, r.rms, r.degenerate, r.converged)
 
+    # ---- relocalisation (include/loam_b200.h "Relocalisation against the whole-run voxel map")
+    def dense_score(self, pts, twists, search_radius=3):
+        """Per pose of twists (K x 6) what dense_align_iterate returns there in n_selected and sum_pd2_sq, all poses in
+        one launch per chunk -> (n_selected int32[K], sum_pd2_sq float32[K])."""
+        a = _pts(pts)
+        poses, k = _poses(twists)
+        sel = np.zeros(max(k, 1), np.int32)
+        ss = np.zeros(max(k, 1), np.float32)
+        self._ck(self.L.loam_b200_dense_score(self.h, _fp(a), a.shape[0], 0, poses, k, int(search_radius), _ip(sel),
+                                              _fp(ss)), "dense_score")
+        return sel[:k].copy(), ss[:k].copy()
+
+    def dense_align_batch(self, pts, twists, search_radius=1, max_iterations=10):
+        """One dense_align per initial pose of twists (K x 6), each equal to the single call -> (K x 6 float32, list of
+        K info dicts as dense_align)."""
+        a = _pts(pts)
+        poses, k = _poses(twists)
+        res = (AlignResult * max(k, 1))()
+        self._ck(self.L.loam_b200_dense_align_batch(self.h, _fp(a), a.shape[0], 0, poses, k, int(search_radius),
+                                                    int(max_iterations), res), "dense_align_batch")
+        outs = [_align_out(list(r.rot) + list(r.pos), r.iterations, r.n_selected, r.rms, r.degenerate, r.converged)
+                for r in res[:k]]
+        return np.array([o[0] for o in outs], np.float32).reshape(k, 6), [o[1] for o in outs]
+
+    def dense_relocalize(self, pts, hypotheses, params=None, cap=16):
+        """Relocalise pts among the hypotheses (K x 6 twists, e.g. reloc_grid) -> ranked candidates (at most cap), each
+        a dict: hypothesis, score_selected, coarse / fine (twist, info) as dense_align, selected, rms."""
+        a = _pts(pts)
+        poses, k = _poses(hypotheses)
+        prm = params if params is not None else RelocParams.default()
+        out = (RelocCandidate * max(int(cap), 1))()
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_relocalize(self.h, _fp(a), a.shape[0], 0, poses, k, C.byref(prm), out,
+                                                   int(cap), C.byref(n)), "dense_relocalize")
+        return [_candidate(r) for r in out[:n.value]]
+
     def profile(self, on=True):
         self.L.loam_b200_profile_enable(self.h, 1 if on else 0)
         self.L.loam_b200_profile_reset(self.h)
@@ -743,6 +809,24 @@ def _align_out(twist, iterations, n_selected, rms, degenerate, converged):
     return np.array(twist, np.float32), {"iterations": int(iterations), "n_selected": int(n_selected),
                                          "rms": np.float32(rms), "degenerate": bool(degenerate),
                                          "converged": bool(converged)}
+
+
+def _poses(twists):
+    """K x 6 twists -> (ctypes Pose array of at least one element, K)."""
+    t = np.ascontiguousarray(twists, np.float32).reshape(-1, 6)
+    poses = (Pose * max(t.shape[0], 1))()
+    for i in range(t.shape[0]):
+        poses[i] = make_pose(t[i])
+    return poses, t.shape[0]
+
+
+def _candidate(r):
+    return {"hypothesis": int(r.hypothesis), "score_selected": int(r.score_selected),
+            "coarse": _align_out(list(r.coarse.rot) + list(r.coarse.pos), r.coarse.iterations, r.coarse.n_selected,
+                                 r.coarse.rms, r.coarse.degenerate, r.coarse.converged),
+            "fine": _align_out(list(r.fine.rot) + list(r.fine.pos), r.fine.iterations, r.fine.n_selected, r.fine.rms,
+                               r.fine.degenerate, r.fine.converged),
+            "selected": int(r.selected), "rms": np.float32(r.rms)}
 
 
 def _ne(ne: NormalEq):
@@ -961,6 +1045,42 @@ class LaserMapping(_Handle):
                  "alignToDenseTarget")
         return _align_out(out, st[0], st[1], rms[0], st[2], st[3])
 
+    def score_dense_target(self, pts, twists, search_radius=3):
+        """BasicLaserMapping::scoreDenseTarget; returns what Ctx.dense_score returns."""
+        a = _pts(pts)
+        t = np.ascontiguousarray(twists, np.float32).reshape(-1, 6)
+        k = t.shape[0]
+        sel = np.zeros(max(k, 1), np.int32)
+        ss = np.zeros(max(k, 1), np.float32)
+        self._ck(self.L.loam_b200_map_dense_score(self.h, _fp(a), a.shape[0], _fp(t), k, int(search_radius), _ip(sel),
+                                                  _fp(ss)), "scoreDenseTarget")
+        return sel[:k].copy(), ss[:k].copy()
+
+    def align_to_dense_target_batch(self, pts, twists, search_radius=1, max_iterations=10):
+        """BasicLaserMapping::alignToDenseTarget over a vector of twists; returns what Ctx.dense_align_batch returns."""
+        a = _pts(pts)
+        t = np.ascontiguousarray(twists, np.float32).reshape(-1, 6)
+        k = t.shape[0]
+        out = np.zeros((max(k, 1), 6), np.float32)
+        st = np.zeros((max(k, 1), 4), np.int32)
+        rms = np.zeros(max(k, 1), np.float32)
+        self._ck(self.L.loam_b200_map_dense_align_batch(self.h, _fp(a), a.shape[0], _fp(t), k, int(search_radius),
+                                                        int(max_iterations), _fp(out), _ip(st), _fp(rms)),
+                 "alignToDenseTarget")
+        infos = [_align_out(out[i], st[i, 0], st[i, 1], rms[i], st[i, 2], st[i, 3])[1] for i in range(k)]
+        return out[:k].copy(), infos
+
+    def relocalize_in_dense_target(self, pts, hypotheses, params=None, cap=16):
+        """BasicLaserMapping::relocalizeInDenseTarget; returns what Ctx.dense_relocalize returns."""
+        a = _pts(pts)
+        t = np.ascontiguousarray(hypotheses, np.float32).reshape(-1, 6)
+        prm = params if params is not None else RelocParams.default()
+        out = (RelocCandidate * max(int(cap), 1))()
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_map_dense_relocalize(self.h, _fp(a), a.shape[0], _fp(t), t.shape[0], C.byref(prm), out,
+                                                       int(cap), C.byref(n)), "relocalizeInDenseTarget")
+        return [_candidate(r) for r in out[:n.value]]
+
     def enable_dense_visibility(self, h_res_deg, v_res_deg, margin):
         """Count, per voxel of the whole-run map, the mapped sweeps that see through it (h_res_deg = 0: off); filter
         with dense_map(max_miss_ratio=...)."""
@@ -1149,6 +1269,29 @@ def gn_solve(AtA, AtB, first_iteration=True, eigen_threshold=10.0):
     if L.loam_b200_host_gn_solve(_fp(a), _fp(b), 1 if first_iteration else 0, eigen_threshold, _fp(x), C.byref(deg)) != 0:
         raise LoamB200Error("gn_solve: invalid arguments")
     return x, bool(deg.value)
+
+
+def reloc_grid(prior6, yaw_step_deg=RELOC_YAW_STEP_DEG, yaw_steps=None, xz_step=RELOC_XZ_STEP,
+               xz_steps=RELOC_XZ_STEPS, sincos=False):
+    """loam_b200_reloc_grid (host only): the relocalisation grid around prior6 -> K x 6 float32 twists, j (yaw) outer,
+    then iz, then ix; yaw_steps None: a full circle, ceil(180 / yaw_step_deg).  sincos=True also returns the poses'
+    cached sin and cos (K x 3 each)."""
+    L = lib()
+    if yaw_steps is None:
+        yaw_steps = int(math.ceil(180.0 / float(np.float32(yaw_step_deg))))
+    prior = make_pose(prior6)
+    n = C.c_int(0)
+    args = (C.byref(prior), np.float32(yaw_step_deg), int(yaw_steps), np.float32(xz_step), int(xz_steps))
+    rc = L.loam_b200_reloc_grid(*args, None, 0, C.byref(n))
+    if rc not in (0, -5):  # LOAM_B200_ERR_CAPACITY: the count is in n
+        raise LoamB200Error(f"reloc_grid: {L.loam_b200_strerror(rc).decode()}")
+    out = (Pose * n.value)()
+    if L.loam_b200_reloc_grid(*args, out, n.value, C.byref(n)) != 0:
+        raise LoamB200Error("reloc_grid failed")
+    tw = np.array([list(p.rot) + list(p.pos) for p in out], np.float32).reshape(-1, 6)
+    if not sincos:
+        return tw
+    return tw, np.array([list(p.sin_) for p in out], np.float32), np.array([list(p.cos_) for p in out], np.float32)
 
 
 def nccl_unique_id() -> bytes:

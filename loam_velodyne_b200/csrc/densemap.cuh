@@ -396,15 +396,87 @@ __global__ void dense_target_gather_kernel(const unsigned long long* __restrict_
 // Slots 0..26 of the 32 sums: AtA (upper triangle) and AtB; 27: selected rows; 28: sum of pd2^2 over them.  The
 // reduction is reduce_normal_equations (fp32 xor butterfly per warp, the 4 warp sums in warp order, CTA partials folded
 // in double in fixed order).  The library is built without FMA contraction, as tests/align_reference.py assumes.
+//
+// Hypotheses (loam_b200_dense_score / _align_batch): blockIdx.y is the entry of the launch's hypothesis list; entry h
+// reads its pose from args[h] and owns partials [h][gridDim.x][stride], result [h][stride] and ticket [h], so one
+// launch evaluates one cloud at every pose of the list and each entry's sums are those of a launch at that pose alone.
+// A single pose is the list of one; the full kernel then takes it by value (LIST = false: the pose `one`, no copy
+// before the launch, read from the parameter bank).  SCORE: only slots 27 and 28 are summed (stride DENSE_SCORE_NEQ), each in the
+// order reduce_normal_equations sums it, so their bits are the full kernel's; the Jacobian row is not formed.
+constexpr int DENSE_SCORE_NEQ = 2;  // the score's slots: selected rows, sum of pd2^2
+
+// reduce_normal_equations restricted to the two score slots (partials and result of stride DENSE_SCORE_NEQ): per slot
+// the same fp32 butterfly, warp order and double fold over the CTA partials, so each slot's bits are that function's
+__device__ __forceinline__ void reduce_score_sums(float n_sel, float sum_sq, float* __restrict__ partials,
+                                                  float* __restrict__ result, unsigned int* ticket, unsigned n_blocks) {
+  __shared__ float s_part[LM_THREADS / 32][DENSE_SCORE_NEQ];
+  __shared__ bool s_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float v0 = n_sel, v1 = sum_sq;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    v0 += __shfl_xor_sync(0xffffffffu, v0, o);
+    v1 += __shfl_xor_sync(0xffffffffu, v1, o);
+  }
+  if (lane == 0) {
+    s_part[warp][0] = v0;
+    s_part[warp][1] = v1;
+  }
+  __syncthreads();
+  if (threadIdx.x < DENSE_SCORE_NEQ) {
+    float v = 0.f;
+    for (int wv = 0; wv < LM_THREADS / 32; wv++) v += s_part[wv][threadIdx.x];
+    __stcg(&partials[(size_t)blockIdx.x * DENSE_SCORE_NEQ + threadIdx.x], v);
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = (atomicAdd(ticket, 1u) == n_blocks - 1);
+  __syncthreads();
+  if (s_last) {
+    __threadfence();
+    __shared__ double s_fold[LM_THREADS / 32][DENSE_SCORE_NEQ];
+    if (lane < DENSE_SCORE_NEQ) {
+      double v = 0.0;
+      for (unsigned bk = warp; bk < n_blocks; bk += LM_THREADS / 32)
+        v += (double)__ldcg(&partials[(size_t)bk * DENSE_SCORE_NEQ + lane]);
+      s_fold[warp][lane] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < DENSE_SCORE_NEQ) {
+      double v = 0.0;
+      for (int wv = 0; wv < LM_THREADS / 32; wv++) v += s_fold[wv][threadIdx.x];
+      result[threadIdx.x] = (float)v;
+    }
+    if (threadIdx.x == 0) *ticket = 0u;
+  }
+}
+
+template <bool SCORE, bool LIST>
 __global__ void __launch_bounds__(LM_THREADS)
 dense_align_kernel(const unsigned long long* __restrict__ skey, const float4* __restrict__ cent,
                    const float4* __restrict__ nrm, int m, float inv, int radius, float gate,
-                   const float4* __restrict__ pts, int n, MapIterArgs a, float* __restrict__ partials,
-                   float* __restrict__ result, unsigned int* ticket, int* __restrict__ dbg_match,
-                   float4* __restrict__ dbg_coeff, int8_t* __restrict__ dbg_sel) {
-  float acc[29];
+                   const float4* __restrict__ pts, int n, MapIterArgs one, const MapIterArgs* __restrict__ args,
+                   float* __restrict__ partials, float* __restrict__ result, unsigned int* ticket,
+                   int* __restrict__ dbg_match, float4* __restrict__ dbg_coeff, int8_t* __restrict__ dbg_sel) {
+  constexpr int NACC = SCORE ? DENSE_SCORE_NEQ : 29;
+  constexpr int SLOT_SEL = SCORE ? 0 : 27, SLOT_SQ = SCORE ? 1 : 28;
+  constexpr int WORDS = (int)(sizeof(MapIterArgs) / sizeof(float));
+  static_assert(WORDS <= LM_THREADS, "one thread per word of the pose");
+  static_assert(LIST || !SCORE, "the score always reads a pose list");
+  __shared__ MapIterArgs s_args;  // LIST: this entry's pose, read from shared memory by every thread
+  if constexpr (LIST) {
+    if (threadIdx.x < WORDS)
+      reinterpret_cast<float*>(&s_args)[threadIdx.x] = reinterpret_cast<const float*>(args + blockIdx.y)[threadIdx.x];
+    __syncthreads();
+  }
+  const MapIterArgs& a = LIST ? s_args : one;  // !LIST: the single pose, a kernel parameter as before the list
+  const int stride = SCORE ? DENSE_SCORE_NEQ : NEQ;
+  partials += (size_t)blockIdx.y * gridDim.x * stride;
+  result += (size_t)blockIdx.y * stride;
+  ticket += blockIdx.y;
+  float acc[NACC];
 #pragma unroll
-  for (int k = 0; k < 29; k++) acc[k] = 0.f;
+  for (int k = 0; k < NACC; k++) acc[k] = 0.f;
   const int i = blockIdx.x * LM_THREADS + threadIdx.x;
   if (i < n) {  // every thread takes part in the reduction below
     const float4 po = pts[i];
@@ -449,27 +521,32 @@ dense_align_kernel(const unsigned long long* __restrict__ skey, const float4* __
         coeff = make_float4(s * nv.x, s * nv.y, s * nv.z, s * pd2);
         sel = (double)s > 0.1;
         if (sel) {
-          float row[6], rhs;
-          map_jacobian_row(a, po, coeff, row, rhs);
-          int k = 0;
+          if constexpr (!SCORE) {
+            float row[6], rhs;
+            map_jacobian_row(a, po, coeff, row, rhs);
+            int k = 0;
 #pragma unroll
-          for (int r = 0; r < 6; r++)
+            for (int r = 0; r < 6; r++)
 #pragma unroll
-            for (int t = r; t < 6; t++) acc[k++] = row[r] * row[t];
+              for (int t = r; t < 6; t++) acc[k++] = row[r] * row[t];
 #pragma unroll
-          for (int r = 0; r < 6; r++) acc[21 + r] = row[r] * rhs;
-          acc[27] = 1.f;
-          acc[28] = pd2 * pd2;
+            for (int r = 0; r < 6; r++) acc[21 + r] = row[r] * rhs;
+          }
+          acc[SLOT_SEL] = 1.f;
+          acc[SLOT_SQ] = pd2 * pd2;
         }
       }
     }
-    if (dbg_match) {
+    if (!SCORE && dbg_match) {  // a single pose only
       dbg_match[i] = best;
       dbg_coeff[i] = coeff;
       dbg_sel[i] = sel ? 1 : 0;
     }
   }
-  reduce_normal_equations(acc, partials, result, ticket, ResultMailbox{nullptr, 0}, gridDim.x);
+  if constexpr (SCORE)
+    reduce_score_sums(acc[0], acc[1], partials, result, ticket, gridDim.x);
+  else
+    reduce_normal_equations(acc, partials, result, ticket, ResultMailbox{nullptr, 0}, gridDim.x);
 }
 
 // ---- visibility pass: one sweep's sensor pose and range image (include/loam_b200.h "loam_b200_dense_visibility")
@@ -604,14 +681,15 @@ struct DenseTarget {
   DevBuf<unsigned long long> keys, keys64;  // sorted keys; load: the entries' keys in input order
   DevBuf<float4> cent, nrm;
   DevBuf<float4> pts;             // the cloud being aligned (a host cloud is uploaded here)
-  DevBuf<float> partials, result; // per-CTA partial sums, the 32 folded sums
-  DevBuf<unsigned> ticket;        // zero between launches (reduce_normal_equations resets it)
+  DevBuf<MapIterArgs> args;       // the poses of one launch's hypothesis list
+  DevBuf<float> partials, result; // per hypothesis: per-CTA partial sums, the folded sums (32, or 2 for a score)
+  DevBuf<unsigned> ticket;        // per hypothesis; zero between launches (the reductions reset it)
   DevBuf<int> match, flag;
   DevBuf<float4> coeff;
   DevBuf<int8_t> sel;
 
   void release() {
-    keys.release(); keys64.release(); cent.release(); nrm.release(); pts.release(); partials.release();
+    keys.release(); keys64.release(); cent.release(); nrm.release(); pts.release(); args.release(); partials.release();
     result.release(); ticket.release(); match.release(); flag.release(); coeff.release(); sel.release();
     n = 0;
     ready = false;

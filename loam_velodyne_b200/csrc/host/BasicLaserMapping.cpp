@@ -8,6 +8,8 @@
 #include <chrono>
 #include <cmath>
 #include <cstring>
+#include <stdexcept>
+#include <string>
 
 #include "b200_runtime.h"
 #include "host_math.h"
@@ -191,6 +193,28 @@ void BasicLaserMapping::loadDenseTarget(float leaf, const pcl::PointCloud<pcl::P
               "loam_b200_dense_target_load");
 }
 
+static Twist twistOf(const float rot[3], const float pos[3]) {
+  Twist t;
+  t.rot_x = rot[0];
+  t.rot_y = rot[1];
+  t.rot_z = rot[2];
+  t.pos.x() = pos[0];
+  t.pos.y() = pos[1];
+  t.pos.z() = pos[2];
+  return t;
+}
+
+static BasicLaserMapping::DenseAlignResult toDenseAlignResult(const loam_b200_align_result& res) {
+  BasicLaserMapping::DenseAlignResult out;
+  out.pose = twistOf(res.rot, res.pos);
+  out.iterations = (size_t)res.iterations;
+  out.nSelected = (size_t)res.n_selected;
+  out.rms = res.rms;
+  out.degenerate = res.degenerate != 0;
+  out.converged = res.converged != 0;
+  return out;
+}
+
 BasicLaserMapping::DenseAlignResult BasicLaserMapping::alignToDenseTarget(const Cloud& cloud, const Twist& initial,
                                                                           int searchRadius, int maxIterations) {
   b200::pack(cloud, _bufA);
@@ -200,18 +224,78 @@ BasicLaserMapping::DenseAlignResult BasicLaserMapping::alignToDenseTarget(const 
   _gpu->check(loam_b200_dense_align(_gpu->get(), _bufA.data(), (int)cloud.points.size(), 0, &pose, searchRadius,
                                     maxIterations, &res),
               "loam_b200_dense_align");
-  DenseAlignResult out;
-  out.pose.rot_x = res.rot[0];
-  out.pose.rot_y = res.rot[1];
-  out.pose.rot_z = res.rot[2];
-  out.pose.pos.x() = res.pos[0];
-  out.pose.pos.y() = res.pos[1];
-  out.pose.pos.z() = res.pos[2];
-  out.iterations = (size_t)res.iterations;
-  out.nSelected = (size_t)res.n_selected;
-  out.rms = res.rms;
-  out.degenerate = res.degenerate != 0;
-  out.converged = res.converged != 0;
+  return toDenseAlignResult(res);
+}
+
+static std::vector<loam_b200_pose> posesOf(const std::vector<Twist>& twists) {
+  std::vector<loam_b200_pose> p(twists.size());
+  for (size_t i = 0; i < twists.size(); i++) b200::fillPose(twists[i], p[i]);
+  return p;
+}
+
+std::vector<BasicLaserMapping::DenseScore> BasicLaserMapping::scoreDenseTarget(const Cloud& cloud,
+                                                                               const std::vector<Twist>& poses,
+                                                                               int searchRadius) {
+  b200::pack(cloud, _bufA);
+  const std::vector<loam_b200_pose> p = posesOf(poses);
+  std::vector<int32_t> sel(poses.size() + 1);
+  std::vector<float> ss(poses.size() + 1);
+  _gpu->check(loam_b200_dense_score(_gpu->get(), _bufA.data(), (int)cloud.points.size(), 0, p.data(), (int)p.size(),
+                                    searchRadius, sel.data(), ss.data()),
+              "loam_b200_dense_score");
+  std::vector<DenseScore> out(poses.size());
+  for (size_t i = 0; i < out.size(); i++) out[i] = DenseScore{(size_t)sel[i], ss[i]};
+  return out;
+}
+
+std::vector<BasicLaserMapping::DenseAlignResult> BasicLaserMapping::alignToDenseTarget(
+    const Cloud& cloud, const std::vector<Twist>& initial, int searchRadius, int maxIterations) {
+  b200::pack(cloud, _bufA);
+  const std::vector<loam_b200_pose> p = posesOf(initial);
+  std::vector<loam_b200_align_result> res(initial.size() + 1);
+  _gpu->check(loam_b200_dense_align_batch(_gpu->get(), _bufA.data(), (int)cloud.points.size(), 0, p.data(),
+                                          (int)p.size(), searchRadius, maxIterations, res.data()),
+              "loam_b200_dense_align_batch");
+  std::vector<DenseAlignResult> out(initial.size());
+  for (size_t i = 0; i < out.size(); i++) out[i] = toDenseAlignResult(res[i]);
+  return out;
+}
+
+std::vector<BasicLaserMapping::RelocCandidate> BasicLaserMapping::relocalizeInDenseTarget(
+    const Cloud& cloud, const std::vector<Twist>& hypotheses, const RelocParams& params, size_t maxCandidates) {
+  b200::pack(cloud, _bufA);
+  const std::vector<loam_b200_pose> p = posesOf(hypotheses);
+  const loam_b200_reloc_params prm{params.scoreRadius, params.coarseRadius, params.fineRadius, params.keep,
+                                   params.maxIterations, params.dedupMetres, params.dedupDegrees};
+  std::vector<loam_b200_reloc_candidate> res(maxCandidates + 1);
+  int n = 0;
+  _gpu->check(loam_b200_dense_relocalize(_gpu->get(), _bufA.data(), (int)cloud.points.size(), 0, p.data(),
+                                         (int)p.size(), &prm, res.data(), (int)maxCandidates, &n),
+              "loam_b200_dense_relocalize");
+  std::vector<RelocCandidate> out((size_t)n);
+  for (int i = 0; i < n; i++) {
+    const loam_b200_reloc_candidate& r = res[(size_t)i];
+    out[(size_t)i] = RelocCandidate{(size_t)r.hypothesis, (size_t)r.score_selected, toDenseAlignResult(r.coarse),
+                                    toDenseAlignResult(r.fine), (size_t)r.selected, r.rms};
+  }
+  return out;
+}
+
+std::vector<Twist> BasicLaserMapping::relocalizationGrid(const Twist& prior, float yawStepDeg, int yawSteps,
+                                                         float xzStep, int xzSteps) {
+  loam_b200_pose p;
+  b200::fillPose(prior, p);
+  int n = 0;
+  int rc = loam_b200_reloc_grid(&p, yawStepDeg, yawSteps, xzStep, xzSteps, nullptr, 0, &n);
+  std::vector<loam_b200_pose> grid;
+  if (rc == LOAM_B200_ERR_CAPACITY) {
+    grid.resize((size_t)n);
+    rc = loam_b200_reloc_grid(&p, yawStepDeg, yawSteps, xzStep, xzSteps, grid.data(), n, &n);
+  }
+  if (rc != LOAM_B200_OK)
+    throw std::runtime_error(std::string("loam_b200_reloc_grid: ") + loam_b200_strerror(rc));
+  std::vector<Twist> out((size_t)n);
+  for (int i = 0; i < n; i++) out[(size_t)i] = twistOf(grid[(size_t)i].rot, grid[(size_t)i].pos);
   return out;
 }
 

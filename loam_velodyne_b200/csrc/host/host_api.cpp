@@ -644,6 +644,100 @@ int loam_b200_map_dense_align(void* h, const float* xyzi, int n, const float* in
     return 0;
   });
 }
+static std::vector<loam::Twist> twists_of(const float* t6, int k) {
+  std::vector<loam::Twist> out((size_t)k);
+  for (int h = 0; h < k; h++) {
+    const float* t = t6 + 6 * h;
+    out[(size_t)h].rot_x = t[0];
+    out[(size_t)h].rot_y = t[1];
+    out[(size_t)h].rot_z = t[2];
+    out[(size_t)h].pos = loam::Vector3(t[3], t[4], t[5]);
+  }
+  return out;
+}
+static void align_result_of(const loam::BasicLaserMapping::DenseAlignResult& r, loam_b200_align_result& o) {
+  o.rot[0] = r.pose.rot_x.rad(); o.rot[1] = r.pose.rot_y.rad(); o.rot[2] = r.pose.rot_z.rad();
+  o.pos[0] = r.pose.pos.x(); o.pos[1] = r.pose.pos.y(); o.pos[2] = r.pose.pos.z();
+  o.iterations = (int)r.iterations;
+  o.n_selected = (int)r.nSelected;
+  o.rms = r.rms;
+  o.degenerate = r.degenerate ? 1 : 0;
+  o.converged = r.converged ? 1 : 0;
+}
+int loam_b200_map_dense_score(void* h, const float* xyzi, int n, const float* poses6, int k, int search_radius,
+                              int* n_selected, float* sum_pd2_sq) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && !xyzi) || !poses6 || k < 1 || !n_selected || !sum_pd2_sq) {
+    g_err = "loam_b200_map_dense_score: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, xyzi, n);
+    const auto r = m->m.scoreDenseTarget(m->scratchA, twists_of(poses6, k), search_radius);
+    for (int i = 0; i < k; i++) {
+      n_selected[i] = (int)r[(size_t)i].nSelected;
+      sum_pd2_sq[i] = r[(size_t)i].sumPd2Sq;
+    }
+    return 0;
+  });
+}
+int loam_b200_map_dense_align_batch(void* h, const float* xyzi, int n, const float* initial6, int k, int search_radius,
+                                    int max_iterations, float* twist_out6, int* stats_out4, float* rms_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && !xyzi) || !initial6 || k < 1 || !twist_out6) {
+    g_err = "loam_b200_map_dense_align_batch: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, xyzi, n);
+    const auto r = m->m.alignToDenseTarget(m->scratchA, twists_of(initial6, k), search_radius, max_iterations);
+    for (int i = 0; i < k; i++) {
+      twist6(r[(size_t)i].pose, twist_out6 + 6 * i);
+      if (stats_out4) {
+        stats_out4[4 * i + 0] = (int)r[(size_t)i].iterations;
+        stats_out4[4 * i + 1] = (int)r[(size_t)i].nSelected;
+        stats_out4[4 * i + 2] = r[(size_t)i].degenerate ? 1 : 0;
+        stats_out4[4 * i + 3] = r[(size_t)i].converged ? 1 : 0;
+      }
+      if (rms_out) rms_out[i] = r[(size_t)i].rms;
+    }
+    return 0;
+  });
+}
+int loam_b200_map_dense_relocalize(void* h, const float* xyzi, int n, const float* hyps6, int k,
+                                   const loam_b200_reloc_params* prm, loam_b200_reloc_candidate* out, int cap,
+                                   int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && !xyzi) || !hyps6 || k < 1 || !prm || !out || cap < 1 || !n_out) {
+    g_err = "loam_b200_map_dense_relocalize: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, xyzi, n);
+    loam::BasicLaserMapping::RelocParams p;
+    p.scoreRadius = prm->score_radius;
+    p.coarseRadius = prm->coarse_radius;
+    p.fineRadius = prm->fine_radius;
+    p.keep = prm->keep;
+    p.maxIterations = prm->max_iterations;
+    p.dedupMetres = prm->dedup_m;
+    p.dedupDegrees = prm->dedup_deg;
+    const auto r = m->m.relocalizeInDenseTarget(m->scratchA, twists_of(hyps6, k), p, (size_t)cap);
+    *n_out = (int)r.size();
+    for (size_t i = 0; i < r.size(); i++) {
+      out[i].hypothesis = (int)r[i].hypothesis;
+      out[i].score_selected = (int)r[i].scoreSelected;
+      align_result_of(r[i].coarse, out[i].coarse);
+      align_result_of(r[i].fine, out[i].fine);
+      out[i].selected = (int)r[i].selected;
+      out[i].rms = r[i].rms;
+    }
+    return 0;
+  });
+}
 int loam_b200_map_debug_dense_table_slots(void* h, long long* out) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;
   return guarded([&] { *out = ((MapH*)h)->m.denseTableSlots(); return 0; });

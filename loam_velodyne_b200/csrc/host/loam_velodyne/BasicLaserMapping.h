@@ -162,6 +162,46 @@ class BasicLaserMapping {
   void loadDenseTarget(float leaf, const pcl::PointCloud<pcl::PointXYZINormal>& target);
   DenseAlignResult alignToDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& cloud, const Twist& initial,
                                       int searchRadius, int maxIterations);
+  // Relocalisation against the target (include/loam_b200.h "Relocalisation against the whole-run voxel map"), for a
+  // restart or a tracking loss with a rough position and no heading.  scoreDenseTarget: per pose the correspondences
+  // and the sum of squared point-to-plane residuals of one alignment iteration there, all poses in one GPU pass.  The
+  // vector overload of alignToDenseTarget runs one independent alignment per initial pose, each equal to the single
+  // call.  relocalizationGrid: a yaw x (x, z) grid around a prior (y is up).  relocalizeInDenseTarget scores the
+  // hypotheses, refines the `keep` best coarse to fine, scores them again, ranks and drops duplicates; candidate 0 is
+  // the answer and its gap to candidate 1 the ambiguity.  Defaults of RelocParams are the recommended parameters.
+  struct DenseScore {
+    size_t nSelected;
+    float sumPd2Sq;
+  };
+  struct RelocParams {
+    RelocParams()
+        : scoreRadius(3), coarseRadius(3), fineRadius(1), keep(16), maxIterations(30), dedupMetres(0.5f),
+          dedupDegrees(5.0f) {}
+    int scoreRadius, coarseRadius, fineRadius;
+    int keep;
+    int maxIterations;
+    float dedupMetres, dedupDegrees;
+  };
+  struct RelocCandidate {
+    size_t hypothesis;     // index into the hypotheses given
+    size_t scoreSelected;  // correspondences at the hypothesis in the first score
+    DenseAlignResult coarse, fine;  // fine.pose is the candidate's pose
+    size_t selected;       // correspondences at fine.pose (fine radius)
+    float rms;             // their point-to-plane RMS
+    const Twist& pose() const { return fine.pose; }
+  };
+  std::vector<DenseScore> scoreDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& cloud,
+                                           const std::vector<Twist>& poses, int searchRadius);
+  std::vector<DenseAlignResult> alignToDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& cloud,
+                                                   const std::vector<Twist>& initial, int searchRadius,
+                                                   int maxIterations);
+  std::vector<RelocCandidate> relocalizeInDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& cloud,
+                                                      const std::vector<Twist>& hypotheses,
+                                                      const RelocParams& params = RelocParams(),
+                                                      size_t maxCandidates = 16);
+  // defaults (the recommended grid): full circle at 2 deg, 0.4 m steps four to each side of the prior (14661 poses)
+  static std::vector<Twist> relocalizationGrid(const Twist& prior, float yawStepDeg = 2.0f, int yawSteps = 90,
+                                               float xzStep = 0.4f, int xzSteps = 4);
 
  private:
   typedef pcl::PointCloud<pcl::PointXYZI> Cloud;

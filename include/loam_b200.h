@@ -567,6 +567,41 @@ int loam_b200_dense_relocalize(loam_b200_ctx* ctx, const float* xyzi, int n, int
                                loam_b200_reloc_candidate* out, int cap, int* n_out);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Ray casting the whole-run voxel map (csrc/densemap.cuh, DESIGN.md "Ray casting the whole-run voxel map"): what the
+ * sensor should see from a pose in the target above -- change detection between sessions, a check of a pose found by
+ * dense_align / dense_relocalize, simulated scans.  Not on the per-sweep path; the result never feeds back into the
+ * mapping stage.  n rays (float[4] in the sensor frame, w ignored: a sweep's own points may be passed; host memory,
+ * or device memory when on_device != 0) from `pose`, fp64 without FMA, each operation rounded on its own, no
+ * transcendental function on the device:
+ *   ray: |p| = sqrt((x*x + y*y) + z*z) in double of the float components, u = p / |p|; d = u rotated into the map frame
+ *     by rotZ, then rotX, then rotY (associate_to_map's order) with std::cos / std::sin in double of the pose's float
+ *     angles; origin o = the pose's float pos as double.  A non-finite or zero p has no hit.
+ *   voxels: L = (double)leaf of the target; voxel v spans [v L, (v + 1) L) per axis; the start voxel is floor(o_a / L);
+ *     a voxel is occupied when its key is in the target (indices outside [-2^20, 2^20) never are).
+ *   walk (Amanatides-Woo with exact re-evaluation): per axis with d_a != 0, inv_a = 1.0 / d_a and t_next_a =
+ *     ((double)k L - o_a) inv_a, k = v_a + 1 when d_a > 0, v_a when d_a < 0; +inf when d_a == 0.  The voxel spans
+ *     [t_enter, t_exit = min t_next), the first one from t_enter = 0.  A step goes along the axis of the smallest t_next
+ *     (ties: x, then y, then z); the next voxel's t_enter is that axis's old t_next, and only its t_next is recomputed,
+ *     from the new index.
+ *   hit: the first occupied voxel with t_exit > min_range; lo = max(t_enter, min_range), hi = t_exit.  With a normal
+ *     (nx not NaN): den = (nx dx + ny dy) + nz dz, num = (nx (cx - ox) + ny (cy - oy)) + nz (cz - oz) with the float
+ *     centroid and normal as double, and t = clamp(num / den, lo, hi) when den != 0; otherwise t = lo.  The surfel
+ *     gives a sub-voxel range on surfaces; the first occupied voxel always stops the ray, so there are no holes.
+ *   out: the walk ends with no hit when t_enter > max_range or the hit's t > max_range.  A hit: range[i] = (float)t,
+ *     index[i] = the voxel's position in the target's ascending key order (the export's order for a built target).
+ *     No hit: range[i] = +inf, index[i] = -1.  index may be NULL.  Synchronous.
+ * A ray index (a hash table of 8^3-voxel bricks with a 512-bit occupancy mask each) is built on the first cast after a
+ * target build or load and kept with the target.  No target: LOAM_B200_ERR_STATE.  LOAM_B200_ERR_ARG unless
+ * 0 <= min_range < max_range (both finite), max_range / leaf <= 65536 (every walk is then at most ~3 * 2^16 steps),
+ * the pose is finite and its position's voxel lies in the key range; and for a NULL pointer.  An empty target or
+ * n = 0 returns no hits and launches nothing.  Launches count under LOAM_B200_K_DENSE.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int loam_b200_dense_raycast(loam_b200_ctx* ctx, const float* rays, int n, int on_device, const loam_b200_pose* pose,
+                            float min_range, float max_range, float* range, int32_t* index);
+/* Test query: device bytes of the target's ray index (0 until the first cast after a build or load). */
+int loam_b200_debug_dense_ray_index_bytes(loam_b200_ctx* ctx, long long* out);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice
  * of the corner and surface queries; with a communicator the 32-float partial normal equations are all-reduced
  * (NCCL, sum, fp32) on the context's stream directly behind the kernel, so every rank returns the same totals and

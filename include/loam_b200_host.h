@@ -137,6 +137,11 @@ int loam_b200_map_dense_align_batch(void* h, const float* xyzi, int n, const flo
 int loam_b200_map_dense_relocalize(void* h, const float* xyzi, int n, const float* hyps6, int k,
                                    const loam_b200_reloc_params* prm, loam_b200_reloc_candidate* out, int cap,
                                    int* n_out);
+/* ray casting that target (BasicLaserMapping::raycastDenseTarget, include/loam_b200.h "Ray casting the whole-run voxel
+ * map"), same in-flight rule: n sensor-frame rays of float[4] from the twist pose6 -> range[n], index[n] (may be
+ * NULL). */
+int loam_b200_map_dense_raycast(void* h, const float* rays, int n, const float* pose6, float min_range,
+                                float max_range, float* range, int* index);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank
  * then enables sharding on its mapping object (nccl_id128 = NULL: slice the queries only, no collective) */
 int loam_b200_host_nccl_unique_id(unsigned char* out128);

@@ -204,6 +204,8 @@ def lib():
                                            C.c_int, _I]),
         "loam_b200_dense_relocalize": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int,
                                                  C.POINTER(RelocParams), C.POINTER(RelocCandidate), C.c_int, _I]),
+        "loam_b200_dense_raycast": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_float, C.c_float, _F, _I]),
+        "loam_b200_debug_dense_ray_index_bytes": (C.c_int, [vp, _LL]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -263,6 +265,7 @@ def lib():
         "loam_b200_map_dense_align_batch": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.c_int, C.c_int, _F, _I, _F]),
         "loam_b200_map_dense_relocalize": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.POINTER(RelocParams),
                                                      C.POINTER(RelocCandidate), C.c_int, _I]),
+        "loam_b200_map_dense_raycast": (C.c_int, [vp, _F, C.c_int, _F, C.c_float, C.c_float, _F, _I]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_map_kernel_profile": (C.c_int, [vp, C.c_int, _D]),
@@ -750,6 +753,30 @@ class Ctx:
                                                    int(cap), C.byref(n)), "dense_relocalize")
         return [_candidate(r) for r in out[:n.value]]
 
+    # ---- ray casting (include/loam_b200.h "Ray casting the whole-run voxel map")
+    def dense_raycast(self, rays, twist6, min_range=0.0, max_range=100.0, on_device=False, n=None):
+        """Cast sensor-frame rays (N x 4, w ignored: lidar_rays() or a sweep's own points) from twist6 into the target
+        -> (range float32[N]: the surfel-refined distance to the first target voxel met within (min_range, max_range],
+        +inf when none; index int32[N]: its position in the target's ascending key order, -1 when none).  With
+        on_device=True, rays is the address of n float[4] in device memory."""
+        p = make_pose(twist6)
+        if on_device:
+            ptr, k = C.cast(C.c_void_p(int(rays)), _F), int(n)
+        else:
+            a = _pts(rays)
+            ptr, k = _fp(a), a.shape[0]
+        rng = np.zeros(max(k, 1), np.float32)
+        idx = np.zeros(max(k, 1), np.int32)
+        self._ck(self.L.loam_b200_dense_raycast(self.h, ptr, k, 1 if on_device else 0, C.byref(p), np.float32(min_range),
+                                                np.float32(max_range), _fp(rng), _ip(idx)), "dense_raycast")
+        return rng[:k].copy(), idx[:k].copy()
+
+    def dense_ray_index_bytes(self):
+        """Test query: device bytes of the target's ray index (0 until the first cast after a build or load)."""
+        out = C.c_longlong(0)
+        self._ck(self.L.loam_b200_debug_dense_ray_index_bytes(self.h, C.byref(out)), "dense_ray_index_bytes")
+        return out.value
+
     def profile(self, on=True):
         self.L.loam_b200_profile_enable(self.h, 1 if on else 0)
         self.L.loam_b200_profile_reset(self.h)
@@ -1081,6 +1108,17 @@ class LaserMapping(_Handle):
                                                        int(cap), C.byref(n)), "relocalizeInDenseTarget")
         return [_candidate(r) for r in out[:n.value]]
 
+    def raycast_dense_target(self, rays, twist6, min_range=0.0, max_range=100.0):
+        """BasicLaserMapping::raycastDenseTarget; returns what Ctx.dense_raycast returns."""
+        a = _pts(rays)
+        t = np.ascontiguousarray(twist6, np.float32).reshape(6)
+        k = a.shape[0]
+        rng = np.zeros(max(k, 1), np.float32)
+        idx = np.zeros(max(k, 1), np.int32)
+        self._ck(self.L.loam_b200_map_dense_raycast(self.h, _fp(a), k, _fp(t), np.float32(min_range),
+                                                    np.float32(max_range), _fp(rng), _ip(idx)), "raycastDenseTarget")
+        return rng[:k].copy(), idx[:k].copy()
+
     def enable_dense_visibility(self, h_res_deg, v_res_deg, margin):
         """Count, per voxel of the whole-run map, the mapped sweeps that see through it (h_res_deg = 0: off); filter
         with dense_map(max_miss_ratio=...)."""
@@ -1292,6 +1330,17 @@ def reloc_grid(prior6, yaw_step_deg=RELOC_YAW_STEP_DEG, yaw_steps=None, xz_step=
     if not sincos:
         return tw
     return tw, np.array([list(p.sin_) for p in out], np.float32), np.array([list(p.cos_) for p in out], np.float32)
+
+
+def lidar_rays(elevations_deg, n_az):
+    """Unit directions of a spinning lidar in the LOAM frame, synth's convention: per elevation e (ring-major), n_az
+    azimuths theta = 2 pi a / n_az, x = -sin(theta) cos(e), y = sin(e), z = cos(theta) cos(e) -> N x 4 float32 (w = 0),
+    the rays of Ctx.dense_raycast."""
+    e = np.radians(np.asarray(elevations_deg, np.float64).reshape(-1))[:, None]
+    theta = 2.0 * math.pi * np.arange(int(n_az), dtype=np.float64)[None, :] / int(n_az)
+    d = np.stack([-np.sin(theta) * np.cos(e), np.broadcast_to(np.sin(e), (e.shape[0], int(n_az))),
+                  np.cos(theta) * np.cos(e), np.zeros((e.shape[0], int(n_az)))], axis=-1)
+    return np.ascontiguousarray(d.reshape(-1, 4), np.float32)
 
 
 def nccl_unique_id() -> bytes:

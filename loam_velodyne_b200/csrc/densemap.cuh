@@ -617,6 +617,186 @@ __global__ void dense_visibility_kernel(DenseSlot* t, unsigned long long size, D
   }
 }
 
+// ---- ray casting the target (include/loam_b200.h "loam_b200_dense_raycast")
+// Ray index: a hash table of 8^3-voxel bricks.  A brick's key is the voxel key >> 3 per axis (bz << 36 | by << 18 | bx);
+// its voxel's local bit is (lz << 6 | ly << 3 | lx).  Built from the target's keys: composite key brick << 9 | bit,
+// sorted (dense_sort64), so each brick's voxels are one run in local-bit order; idx[j] = the target index of sorted
+// position j, and a brick's slot keeps its 512-bit mask and the position of its run's head.  A voxel's target index
+// is then idx[base + popc(mask below its bit)].
+constexpr int DENSE_BRICK_WORDS = 8;                 // 64-bit words of a brick's mask
+constexpr int DENSE_RAY_MAX_STEPS = 3 * 65536 + 4;   // max_range / leaf <= 65536 crosses at most sqrt(3) 65536 + 3 faces
+
+struct DenseRayIndex {                 // device view, by value in the kernel arguments
+  const unsigned long long* key;       // brick key per slot, DENSE_EMPTY when free
+  const unsigned long long* mask;      // DENSE_BRICK_WORDS words per slot
+  const unsigned* base;                // per slot: sorted position of the brick's first voxel
+  const int* idx;                      // per sorted position: target index
+  unsigned long long slots_mask;       // slots - 1 (a power of two)
+};
+
+struct DenseRayArgs {                  // by value in the kernel arguments
+  double ox, oy, oz;                   // origin: the pose's float pos
+  double cx, sx, cy, sy, cz, sz;       // std::cos / std::sin of the pose's float rot_x, rot_y, rot_z (host)
+  double leaf, min_range, max_range;
+};
+
+__device__ __forceinline__ unsigned long long dense_brick_composite(unsigned long long key) {
+  const unsigned long long vx = key & DENSE_AXIS_MASK, vy = (key >> 21) & DENSE_AXIS_MASK, vz = key >> 42;
+  const unsigned long long brick = ((vz >> 3) << 36) | ((vy >> 3) << 18) | (vx >> 3);
+  return (brick << 9) | ((vz & 7) << 6) | ((vy & 7) << 3) | (vx & 7);
+}
+
+// composite keys of the target's voxels + the (low word, index) pairs of the first sort pass
+__global__ void dense_brick_key_kernel(const unsigned long long* __restrict__ keys, int n,
+                                       unsigned long long* __restrict__ comp, unsigned* __restrict__ keys_lo,
+                                       int* __restrict__ vals) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long c = dense_brick_composite(keys[i]);
+  comp[i] = c;
+  keys_lo[i] = (unsigned)c;
+  vals[i] = i;
+}
+
+// per sorted position: keep the target index, count the bricks (run heads)
+__global__ void dense_brick_count_kernel(const unsigned long long* __restrict__ comp, const int* __restrict__ order,
+                                         int n, int* __restrict__ idx, int* __restrict__ bricks) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int o = order[j];
+  idx[j] = o;
+  if (j == 0 || (comp[o] >> 9) != (comp[order[j - 1]] >> 9)) atomicAdd(bricks, 1);
+}
+
+// per sorted position: find or claim the brick's slot (load factor <= 0.5), set the voxel's bit; the head sets base
+__global__ void dense_brick_fill_kernel(const unsigned long long* __restrict__ comp, const int* __restrict__ idx, int n,
+                                        unsigned long long* bkey, unsigned long long* bmask, unsigned* __restrict__ bbase,
+                                        unsigned long long smask) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const unsigned long long c = comp[idx[j]], brick = c >> 9;
+  const unsigned bit = (unsigned)(c & 511);
+  unsigned long long h = dense_hash(brick) & smask;
+  for (;;) {
+    const unsigned long long prev = atomicCAS(&bkey[h], DENSE_EMPTY, brick);
+    if (prev == DENSE_EMPTY || prev == brick) break;
+    h = (h + 1) & smask;
+  }
+  atomicOr(&bmask[h * DENSE_BRICK_WORDS + (bit >> 6)], 1ull << (bit & 63));
+  if (j == 0 || (comp[idx[j - 1]] >> 9) != brick) bbase[h] = (unsigned)j;
+}
+
+// slot of the brick holding voxel (vx, vy, vz), -1 when the brick is empty or the voxel outside the key range
+__device__ __forceinline__ long long dense_brick_find(const DenseRayIndex& ix, int vx, int vy, int vz) {
+  constexpr int H = 1 << 20;
+  if (vx < -H || vx >= H || vy < -H || vy >= H || vz < -H || vz >= H) return -1;
+  const unsigned long long brick = ((unsigned long long)((vz + H) >> 3) << 36) |
+                                   ((unsigned long long)((vy + H) >> 3) << 18) | (unsigned long long)((vx + H) >> 3);
+  unsigned long long h = dense_hash(brick) & ix.slots_mask;
+  for (;;) {
+    const unsigned long long k = __ldg(&ix.key[h]);
+    if (k == brick) return (long long)h;
+    if (k == DENSE_EMPTY) return -1;
+    h = (h + 1) & ix.slots_mask;
+  }
+}
+
+__device__ __forceinline__ unsigned dense_local_bit(int vx, int vy, int vz) {
+  constexpr int H = 1 << 20;
+  return ((unsigned)((vz + H) & 7) << 6) | ((unsigned)((vy + H) & 7) << 3) | (unsigned)((vx + H) & 7);
+}
+
+// One thread per ray (tests/raycast_reference.py restates it), fp64 without FMA, each operation rounded on its own:
+//   |p| = sqrt((x*x + y*y) + z*z) of the float components; u = p / |p|; d = rotZ, rotX, rotY of u (to_map64's order);
+//   a non-finite or zero p has no hit.  Start voxel floor(o_a / L); per axis with d_a != 0 inv_a = 1 / d_a and
+//   t_next_a = ((double)k * L - o_a) * inv_a with k = v_a + 1 (d_a > 0) or v_a (d_a < 0); +inf when d_a == 0.
+//   Per voxel [t_enter, t_exit = min t_next): stop when t_enter > max_range; the first occupied voxel with
+//   t_exit > min_range is the hit, at t = clamp(num / den, lo, hi) on its surfel (den != 0) or lo (no normal, or
+//   den == 0), lo = max(t_enter, min_range), hi = t_exit; t > max_range is no hit.  Then one step along the axis of the
+//   smallest t_next (ties x, y, z); t_enter = its old t_next; only its t_next is recomputed, from the new index.
+// The mask word is read per voxel only inside a non-empty brick; the hash is probed once per brick entered.
+__global__ void
+dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, DenseRayIndex ix,
+                     const float4* __restrict__ cent, const float4* __restrict__ nrm, float* __restrict__ range,
+                     int* __restrict__ index) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 p = rays[i];
+  const double px = (double)p.x, py = (double)p.y, pz = (double)p.z;
+  const double len = sqrt((px * px + py * py) + pz * pz);
+  if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && len > 0.0) {
+    const double ux = px / len, uy = py / len, uz = pz / len;
+    const double x1 = a.cz * ux - a.sz * uy, y1 = a.sz * ux + a.cz * uy;
+    const double y2 = a.cx * y1 - a.sx * uz, z2 = a.sx * y1 + a.cx * uz;
+    const double dx = a.cy * x1 + a.sy * z2, dy = y2, dz = a.cy * z2 - a.sy * x1;
+    const double L = a.leaf, inf = __longlong_as_double(0x7ff0000000000000ll);
+    int vx = (int)floor(a.ox / L), vy = (int)floor(a.oy / L), vz = (int)floor(a.oz / L);
+    const int stx = dx > 0.0 ? 1 : -1, sty = dy > 0.0 ? 1 : -1, stz = dz > 0.0 ? 1 : -1;
+    const double ivx = 1.0 / dx, ivy = 1.0 / dy, ivz = 1.0 / dz;
+    double tnx = dx != 0.0 ? ((double)(dx > 0.0 ? vx + 1 : vx) * L - a.ox) * ivx : inf;
+    double tny = dy != 0.0 ? ((double)(dy > 0.0 ? vy + 1 : vy) * L - a.oy) * ivy : inf;
+    double tnz = dz != 0.0 ? ((double)(dz > 0.0 ? vz + 1 : vz) * L - a.oz) * ivz : inf;
+    double t_enter = 0.0, lo = 0.0, hi = 0.0;
+    int j_hit = -1;
+    long long slot = dense_brick_find(ix, vx, vy, vz);
+    for (int s = 0; s < DENSE_RAY_MAX_STEPS; s++) {
+      if (t_enter > a.max_range) break;
+      const int ax = (tnx <= tny && tnx <= tnz) ? 0 : (tny <= tnz ? 1 : 2);
+      const double t_exit = ax == 0 ? tnx : (ax == 1 ? tny : tnz);
+      if (slot >= 0 && t_exit > a.min_range) {
+        const unsigned bit = dense_local_bit(vx, vy, vz);
+        const unsigned long long* m = ix.mask + slot * DENSE_BRICK_WORDS;
+        const unsigned long long w = __ldg(&m[bit >> 6]);
+        if ((w >> (bit & 63)) & 1ull) {
+          int below = __popcll(w & ((1ull << (bit & 63)) - 1ull));
+          for (unsigned k = 0; k < (bit >> 6); k++) below += __popcll(__ldg(&m[k]));
+          j_hit = __ldg(&ix.idx[__ldg(&ix.base[slot]) + below]);
+          lo = t_enter > a.min_range ? t_enter : a.min_range;
+          hi = t_exit;
+          break;
+        }
+      }
+      t_enter = t_exit;
+      bool crossed;
+      if (ax == 0) {
+        vx += stx;
+        tnx = ((double)(stx > 0 ? vx + 1 : vx) * L - a.ox) * ivx;
+        crossed = ((vx + (1 << 20)) & 7) == (stx > 0 ? 0 : 7);
+      } else if (ax == 1) {
+        vy += sty;
+        tny = ((double)(sty > 0 ? vy + 1 : vy) * L - a.oy) * ivy;
+        crossed = ((vy + (1 << 20)) & 7) == (sty > 0 ? 0 : 7);
+      } else {
+        vz += stz;
+        tnz = ((double)(stz > 0 ? vz + 1 : vz) * L - a.oz) * ivz;
+        crossed = ((vz + (1 << 20)) & 7) == (stz > 0 ? 0 : 7);
+      }
+      if (crossed) slot = dense_brick_find(ix, vx, vy, vz);
+    }
+    if (j_hit >= 0) {  // the surfel range, outside the walk (its division stays out of the loop)
+      double t = lo;
+      const float4 nv = nrm[j_hit];
+      if (!isnan(nv.x)) {
+        const double den = ((double)nv.x * dx + (double)nv.y * dy) + (double)nv.z * dz;
+        if (den != 0.0) {
+          const float4 c = cent[j_hit];
+          const double num = ((double)nv.x * ((double)c.x - a.ox) + (double)nv.y * ((double)c.y - a.oy)) +
+                             (double)nv.z * ((double)c.z - a.oz);
+          const double q = num / den;
+          t = q < lo ? lo : (q > hi ? hi : q);
+        }
+      }
+      if (!(t > a.max_range)) {
+        range[i] = (float)t;
+        index[i] = j_hit;
+        return;
+      }
+    }
+  }
+  range[i] = __int_as_float(0x7f800000);  // no hit
+  index[i] = -1;
+}
+
 // Host-side state of the map (loam_b200_ctx::dense).  The insertion runs on its own stream with its own sort scratch,
 // so the next sweep's stages on the main stream and the map update on its lanes neither wait for it nor share buffers.
 struct DenseMap {
@@ -687,10 +867,20 @@ struct DenseTarget {
   DevBuf<int> match, flag;
   DevBuf<float4> coeff;
   DevBuf<int8_t> sel;
+  // ray index of loam_b200_dense_raycast: built on the first cast after a build or load (ray_slots > 0 once built)
+  unsigned long long ray_slots = 0;
+  DevBuf<unsigned long long> ray_key, ray_mask;
+  DevBuf<unsigned> ray_base;
+  DevBuf<int> ray_idx;
+  DevBuf<float> ray_range;        // the cast's outputs
+  DevBuf<int> ray_hit;
 
   void release() {
     keys.release(); keys64.release(); cent.release(); nrm.release(); pts.release(); args.release(); partials.release();
     result.release(); ticket.release(); match.release(); flag.release(); coeff.release(); sel.release();
+    ray_key.release(); ray_mask.release(); ray_base.release(); ray_idx.release(); ray_range.release();
+    ray_hit.release();
+    ray_slots = 0;
     n = 0;
     ready = false;
   }

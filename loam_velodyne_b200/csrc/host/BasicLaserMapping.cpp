@@ -281,6 +281,20 @@ std::vector<BasicLaserMapping::RelocCandidate> BasicLaserMapping::relocalizeInDe
   return out;
 }
 
+void BasicLaserMapping::raycastDenseTarget(const Cloud& rays, const Twist& pose, float minRange, float maxRange,
+                                           std::vector<float>& range, std::vector<int>* index) {
+  b200::pack(rays, _bufA);
+  loam_b200_pose p;
+  b200::fillPose(pose, p);
+  const size_t n = rays.points.size();
+  range.resize(n);
+  std::vector<int32_t> idx(index ? n : 0);
+  _gpu->check(loam_b200_dense_raycast(_gpu->get(), _bufA.data(), (int)n, 0, &p, minRange, maxRange, range.data(),
+                                      index ? idx.data() : nullptr),
+              "loam_b200_dense_raycast");
+  if (index) index->assign(idx.begin(), idx.end());
+}
+
 std::vector<Twist> BasicLaserMapping::relocalizationGrid(const Twist& prior, float yawStepDeg, int yawSteps,
                                                          float xzStep, int xzSteps) {
   loam_b200_pose p;

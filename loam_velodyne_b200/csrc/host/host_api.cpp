@@ -738,6 +738,24 @@ int loam_b200_map_dense_relocalize(void* h, const float* xyzi, int n, const floa
     return 0;
   });
 }
+int loam_b200_map_dense_raycast(void* h, const float* rays, int n, const float* pose6, float min_range,
+                                float max_range, float* range, int* index) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && (!rays || !range)) || !pose6) {
+    g_err = "loam_b200_map_dense_raycast: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, rays, n);
+    std::vector<float> r;
+    std::vector<int> idx;
+    m->m.raycastDenseTarget(m->scratchA, twists_of(pose6, 1)[0], min_range, max_range, r, index ? &idx : nullptr);
+    if (n > 0) std::memcpy(range, r.data(), (size_t)n * sizeof(float));
+    if (index && n > 0) std::memcpy(index, idx.data(), (size_t)n * sizeof(int));
+    return 0;
+  });
+}
 int loam_b200_map_debug_dense_table_slots(void* h, long long* out) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;
   return guarded([&] { *out = ((MapH*)h)->m.denseTableSlots(); return 0; });

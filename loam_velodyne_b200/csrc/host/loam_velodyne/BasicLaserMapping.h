@@ -202,6 +202,12 @@ class BasicLaserMapping {
   // defaults (the recommended grid): full circle at 2 deg, 0.4 m steps four to each side of the prior (14661 poses)
   static std::vector<Twist> relocalizationGrid(const Twist& prior, float yawStepDeg = 2.0f, int yawSteps = 90,
                                                float xzStep = 0.4f, int xzSteps = 4);
+  // Ray casting the target (include/loam_b200.h "Ray casting the whole-run voxel map"): what the sensor should see
+  // from `pose`.  Each point of `rays` is a direction in the sensor frame (a sweep's own points may be passed); range[i]
+  // is the surfel-refined distance to the first target voxel the ray meets within (minRange, maxRange], +inf when
+  // none; index (optional) its position in the target, -1 when none.
+  void raycastDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& rays, const Twist& pose, float minRange,
+                          float maxRange, std::vector<float>& range, std::vector<int>* index = nullptr);
 
  private:
   typedef pcl::PointCloud<pcl::PointXYZI> Cloud;

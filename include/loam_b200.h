@@ -382,7 +382,20 @@ int loam_b200_debug_tree_build_path(loam_b200_ctx* ctx, int slot);
  *           the map (or on a sharded context) LOAM_B200_ERR_STATE.
  *   observe: the pass over the cloud in any slot (map frame) seen from `pose` (kernel-level use and tests; the mapping
  *           stage observes MAP_FULL itself); everything enqueued on the context afterwards waits for it.
- *           LOAM_B200_ERR_STATE while the pass is off.
+ *           LOAM_B200_ERR_STATE while the pass is off (in both modes).  It runs whichever mode is on.
+ *   carving: the pass's other mode, carve mode (DESIGN.md "Carve mode"), instead of the range image: each mapped sweep,
+ *           at the same place, walks every point's ray from the pose's float position o through the map, fp64 without
+ *           FMA: e = p - o per axis, r = sqrt((ex*ex + ey*ey) + ez*ez), d = e / r (a non-finite p or r == 0, or an
+ *           origin whose voxel lies outside the key range, casts nothing); the walk of loam_b200_dense_raycast from o
+ *           along d (start voxel floor(o_a / leaf), ties x, y, z); T = min(r - margin, max_range); the walk ends at the
+ *           first voxel with t_exit > T, and each voxel before it that is stored (before the sweep's insertion) is
+ *           carved.  K = the voxels of the sweep's own points by the map's rule.  Every stored voxel carved by at least
+ *           one ray and not in K gets one miss per sweep (hits win within a sweep), independent of thread order and of
+ *           how many rays crossed it.  Cost: O(rays x voxels walked), independent of the map's size; an occupancy
+ *           index of 8^3 bricks kept current by the insertion replaces any pass over the table.  max_range == 0 turns
+ *           it off.  LOAM_B200_ERR_ARG unless margin >= 0 and max_range >= 0 are finite and max_range / leaf <= 65536.
+ *           Without the map (or on a sharded context) LOAM_B200_ERR_STATE.  The two modes exclude each other: turning
+ *           one on while the other is on gives LOAM_B200_ERR_STATE.  Misses saturate and feed the exports as above.
  *   export_filtered: the voxels with (double) misses <= max_miss_ratio * (double) hits (max_miss_ratio >= 0; +inf
  *           keeps every voxel and equals loam_b200_dense_export), in ascending voxel order, with the same centroids;
  *           counts, hits and misses may each be NULL.  *n_out = number of voxels kept, LOAM_B200_ERR_CAPACITY when it
@@ -415,6 +428,7 @@ int loam_b200_dense_export(loam_b200_ctx* ctx, float* xyzi, uint32_t* counts, in
 int loam_b200_dense_clear(loam_b200_ctx* ctx);
 int loam_b200_dense_visibility(loam_b200_ctx* ctx, double h_res_deg, double v_res_deg, double margin);
 int loam_b200_dense_observe(loam_b200_ctx* ctx, int slot, const loam_b200_pose* pose);
+int loam_b200_dense_carving(loam_b200_ctx* ctx, double margin, double max_range);
 int loam_b200_dense_export_filtered(loam_b200_ctx* ctx, double max_miss_ratio, float* xyzi, uint32_t* counts,
                                     uint16_t* hits, uint16_t* misses, int cap, int* n_out);
 int loam_b200_dense_export_normals(loam_b200_ctx* ctx, double max_miss_ratio, int radius, const double viewpoint[3],
@@ -422,6 +436,10 @@ int loam_b200_dense_export_normals(loam_b200_ctx* ctx, double max_miss_ratio, in
 /* Test query: slots of the map's hash table as the host sized it last (0 while the map is off).  The table keeps a
  * load factor <= 0.5 of an upper bound of the voxels, so it follows the voxels stored, not the points inserted. */
 int loam_b200_debug_dense_table_slots(loam_b200_ctx* ctx, long long* out);
+/* Test query: carve mode's occupancy index as rows of 9 words (brick key (v >> 3 per axis of v + 2^20: z << 36 |
+ * y << 18 | x), then the 512-bit mask of its voxels, bit (z & 7) << 6 | (y & 7) << 3 | (x & 7)) in ascending brick key;
+ * *n_out = its bricks, LOAM_B200_ERR_CAPACITY when they exceed cap rows.  0 bricks while there is no index. */
+int loam_b200_debug_dense_carve_index(loam_b200_ctx* ctx, uint64_t* rows, long long cap, long long* n_out);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Alignment against the whole-run voxel map (csrc/densemap.cuh, DESIGN.md "Alignment against the whole-run voxel map"):

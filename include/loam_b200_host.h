@@ -106,6 +106,9 @@ int loam_b200_map_dense_clear(void* h);
  * export filtered by max_miss_ratio (BasicLaserMapping::denseMapFiltered): as loam_b200_map_dense_export,
  * plus per-voxel hits / misses when non-NULL.  Same in-flight rule as the four above. */
 int loam_b200_map_dense_visibility(void* h, double h_res_deg, double v_res_deg, double margin);
+/* carve mode of the pass (BasicLaserMapping::enableDenseCarving, include/loam_b200.h "loam_b200_dense_carving");
+ * max_range 0 turns it off.  Same in-flight rule. */
+int loam_b200_map_dense_carving(void* h, double margin, double max_range);
 int loam_b200_map_dense_export_filtered(void* h, double max_miss_ratio, float* xyzi, unsigned int* counts,
                                         unsigned short* hits, unsigned short* misses, int cap, int* n_out);
 /* the filtered export with a normal and curvature per voxel (BasicLaserMapping::denseMapNormals, include/loam_b200.h

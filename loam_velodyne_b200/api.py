@@ -109,6 +109,8 @@ _U = C.POINTER(C.c_uint32)
 _U16 = C.POINTER(C.c_uint16)
 _LL = C.POINTER(C.c_longlong)
 DENSE_MAX_VOXELS = 2**31 - 1  # default cap of the whole-run voxel map: none below the export's int32 count
+# recommended carve mode parameters (DESIGN.md "Carve mode"): margin in metres, maximum range in metres
+DENSE_CARVE_MARGIN, DENSE_CARVE_MAX_RANGE = 2.0, 100.0
 
 _lib = None
 
@@ -188,9 +190,11 @@ def lib():
         "loam_b200_dense_clear": (C.c_int, [vp]),
         "loam_b200_dense_visibility": (C.c_int, [vp, C.c_double, C.c_double, C.c_double]),
         "loam_b200_dense_observe": (C.c_int, [vp, C.c_int, C.POINTER(Pose)]),
+        "loam_b200_dense_carving": (C.c_int, [vp, C.c_double, C.c_double]),
         "loam_b200_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
         "loam_b200_dense_export_normals": (C.c_int, [vp, C.c_double, C.c_int, _D, _F, _U, _F, C.c_int, _I]),
         "loam_b200_debug_dense_table_slots": (C.c_int, [vp, _LL]),
+        "loam_b200_debug_dense_carve_index": (C.c_int, [vp, C.POINTER(C.c_uint64), C.c_longlong, _LL]),
         "loam_b200_dense_target_build": (C.c_int, [vp, C.c_double, C.c_int, _D, _I]),
         "loam_b200_dense_target_load": (C.c_int, [vp, C.c_float, _F, _F, C.c_int]),
         "loam_b200_dense_align_iterate": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int,
@@ -255,6 +259,7 @@ def lib():
         "loam_b200_map_dense_export": (C.c_int, [vp, _F, _U, C.c_int, _I]),
         "loam_b200_map_dense_clear": (C.c_int, [vp]),
         "loam_b200_map_dense_visibility": (C.c_int, [vp, C.c_double, C.c_double, C.c_double]),
+        "loam_b200_map_dense_carving": (C.c_int, [vp, C.c_double, C.c_double]),
         "loam_b200_map_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
         "loam_b200_map_dense_export_normals": (C.c_int, [vp, C.c_double, C.c_int, _D, _F, _U, _F, C.c_int, _I]),
         "loam_b200_map_debug_dense_table_slots": (C.c_int, [vp, _LL]),
@@ -663,6 +668,23 @@ class Ctx:
         one miss for every stored voxel the cloud sees through."""
         p = make_pose(twist6)
         self._ck(self.L.loam_b200_dense_observe(self.h, slot, C.byref(p)), "dense_observe")
+
+    def dense_carving(self, margin=DENSE_CARVE_MARGIN, max_range=DENSE_CARVE_MAX_RANGE):
+        """Carve mode of the visibility pass instead of the range image (max_range = 0: off): every point's ray is walked
+        from the pose through the map, and each stored voxel it crosses up to min(r - margin, max_range), and that no
+        point of the cloud falls into, gets one miss per observed cloud.  See dense_observe."""
+        self._ck(self.L.loam_b200_dense_carving(self.h, float(margin), float(max_range)), "dense_carving")
+
+    def dense_carve_index(self):
+        """Test query: carve mode's occupancy index -> (brick keys B uint64 ascending, masks B x 8 uint64)."""
+        n = C.c_longlong(0)
+        rc = self.L.loam_b200_debug_dense_carve_index(self.h, None, 0, C.byref(n))
+        if rc not in (0, -5):  # LOAM_B200_ERR_CAPACITY: the count is in n
+            self._ck(rc, "dense_carve_index")
+        rows = np.zeros((n.value, 9), np.uint64)
+        self._ck(self.L.loam_b200_debug_dense_carve_index(self.h, rows.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                          n.value, C.byref(n)), "dense_carve_index")
+        return rows[:, 0].copy(), rows[:, 1:].copy()
 
     def dense_clear(self):
         self._ck(self.L.loam_b200_dense_clear(self.h), "dense_clear")
@@ -1124,6 +1146,11 @@ class LaserMapping(_Handle):
         with dense_map(max_miss_ratio=...)."""
         self._ck(self.L.loam_b200_map_dense_visibility(self.h, float(h_res_deg), float(v_res_deg), float(margin)),
                  "enableDenseVisibility")
+
+    def enable_dense_carving(self, margin=DENSE_CARVE_MARGIN, max_range=DENSE_CARVE_MAX_RANGE):
+        """The visibility pass in carve mode: each mapped sweep's rays give one miss to every stored voxel they cross
+        (max_range = 0: off; the range-image mode must be off); filter with dense_map(max_miss_ratio=...)."""
+        self._ck(self.L.loam_b200_map_dense_carving(self.h, float(margin), float(max_range)), "enableDenseCarving")
 
     def clear_dense_map(self):
         self._ck(self.L.loam_b200_map_dense_clear(self.h), "clearDenseMap")

@@ -15,7 +15,9 @@
 //   room under max_voxels) -> counters.
 // Every insert also counts a hit for each voxel that receives points.  The optional visibility pass (before a sweep's
 // insert, dense_range_image_kernel + dense_visibility_kernel) counts a miss for every stored voxel that the sweep sees
-// through: its pixel of the sweep's range image holds a return farther than the centroid's range + margin.
+// through: its pixel of the sweep's range image holds a return farther than the centroid's range + margin.  Its other
+// mode, carve mode (dense_carve_mark_kernel + dense_carve_kernel), walks every point's ray through a live occupancy
+// index of the table instead and counts one miss for every stored voxel a ray crosses short of its return.
 // Per voxel the table keeps count and the fp64 sums S = ((P1 + P2) + P3) + ... of the per-sweep partial sums; export
 // gives (float)(S / count) per field in ascending key order, so the result does not depend on where the hash placed
 // an entry.  Keys are unique within one insert, so no value update needs an atomic.
@@ -44,6 +46,7 @@ __device__ __forceinline__ unsigned dense_add_miss(unsigned e) { return (e >> 16
 
 struct DenseCounters {
   unsigned long long voxels, skipped, dropped;
+  unsigned long long bricks;  // bricks of carve mode's occupancy index (0 while carve mode is off)
 };
 
 // per-run results of one insert (indexed by run = voxel rank in key order)
@@ -706,10 +709,53 @@ __device__ __forceinline__ unsigned dense_local_bit(int vx, int vy, int vz) {
   return ((unsigned)((vz + H) & 7) << 6) | ((unsigned)((vy + H) & 7) << 3) | (unsigned)((vx + H) & 7);
 }
 
+// The voxel walk of a ray from o along d (Amanatides-Woo), shared by the ray cast and carve mode, fp64 without FMA:
+// start voxel floor(o_a / L); per axis with d_a != 0 inv_a = 1 / d_a and t_next_a = ((double)k * L - o_a) * inv_a with
+// k = v_a + 1 (d_a > 0) or v_a (d_a < 0); +inf when d_a == 0.  The current voxel spans [t_enter, t_exit = min t_next);
+// step() moves along axis() -- the smallest t_next, ties x, y, z -- and recomputes only that axis's t_next, from its new
+// index, so no error accumulates.  It returns whether the step entered another 8^3 brick.
+struct DenseWalk {
+  double ox, oy, oz, L, ivx, ivy, ivz, tnx, tny, tnz;
+  int vx, vy, vz, stx, sty, stz;
+
+  __device__ __forceinline__ DenseWalk(double ox_, double oy_, double oz_, double dx, double dy, double dz, double L_)
+      : ox(ox_), oy(oy_), oz(oz_), L(L_) {
+    const double inf = __longlong_as_double(0x7ff0000000000000ll);
+    vx = (int)floor(ox / L);
+    vy = (int)floor(oy / L);
+    vz = (int)floor(oz / L);
+    stx = dx > 0.0 ? 1 : -1;
+    sty = dy > 0.0 ? 1 : -1;
+    stz = dz > 0.0 ? 1 : -1;
+    ivx = 1.0 / dx;
+    ivy = 1.0 / dy;
+    ivz = 1.0 / dz;
+    tnx = dx != 0.0 ? ((double)(dx > 0.0 ? vx + 1 : vx) * L - ox) * ivx : inf;
+    tny = dy != 0.0 ? ((double)(dy > 0.0 ? vy + 1 : vy) * L - oy) * ivy : inf;
+    tnz = dz != 0.0 ? ((double)(dz > 0.0 ? vz + 1 : vz) * L - oz) * ivz : inf;
+  }
+  __device__ __forceinline__ int axis() const { return (tnx <= tny && tnx <= tnz) ? 0 : (tny <= tnz ? 1 : 2); }
+  __device__ __forceinline__ double t_next(int ax) const { return ax == 0 ? tnx : (ax == 1 ? tny : tnz); }
+  __device__ __forceinline__ bool step(int ax) {
+    if (ax == 0) {
+      vx += stx;
+      tnx = ((double)(stx > 0 ? vx + 1 : vx) * L - ox) * ivx;
+      return ((vx + (1 << 20)) & 7) == (stx > 0 ? 0 : 7);
+    }
+    if (ax == 1) {
+      vy += sty;
+      tny = ((double)(sty > 0 ? vy + 1 : vy) * L - oy) * ivy;
+      return ((vy + (1 << 20)) & 7) == (sty > 0 ? 0 : 7);
+    }
+    vz += stz;
+    tnz = ((double)(stz > 0 ? vz + 1 : vz) * L - oz) * ivz;
+    return ((vz + (1 << 20)) & 7) == (stz > 0 ? 0 : 7);
+  }
+};
+
 // One thread per ray (tests/raycast_reference.py restates it), fp64 without FMA, each operation rounded on its own:
 //   |p| = sqrt((x*x + y*y) + z*z) of the float components; u = p / |p|; d = rotZ, rotX, rotY of u (to_map64's order);
-//   a non-finite or zero p has no hit.  Start voxel floor(o_a / L); per axis with d_a != 0 inv_a = 1 / d_a and
-//   t_next_a = ((double)k * L - o_a) * inv_a with k = v_a + 1 (d_a > 0) or v_a (d_a < 0); +inf when d_a == 0.
+//   a non-finite or zero p has no hit.  The walk is DenseWalk's.
 //   Per voxel [t_enter, t_exit = min t_next): stop when t_enter > max_range; the first occupied voxel with
 //   t_exit > min_range is the hit, at t = clamp(num / den, lo, hi) on its surfel (den != 0) or lo (no normal, or
 //   den == 0), lo = max(t_enter, min_range), hi = t_exit; t > max_range is no hit.  Then one step along the axis of the
@@ -729,22 +775,16 @@ dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, Den
     const double x1 = a.cz * ux - a.sz * uy, y1 = a.sz * ux + a.cz * uy;
     const double y2 = a.cx * y1 - a.sx * uz, z2 = a.sx * y1 + a.cx * uz;
     const double dx = a.cy * x1 + a.sy * z2, dy = y2, dz = a.cy * z2 - a.sy * x1;
-    const double L = a.leaf, inf = __longlong_as_double(0x7ff0000000000000ll);
-    int vx = (int)floor(a.ox / L), vy = (int)floor(a.oy / L), vz = (int)floor(a.oz / L);
-    const int stx = dx > 0.0 ? 1 : -1, sty = dy > 0.0 ? 1 : -1, stz = dz > 0.0 ? 1 : -1;
-    const double ivx = 1.0 / dx, ivy = 1.0 / dy, ivz = 1.0 / dz;
-    double tnx = dx != 0.0 ? ((double)(dx > 0.0 ? vx + 1 : vx) * L - a.ox) * ivx : inf;
-    double tny = dy != 0.0 ? ((double)(dy > 0.0 ? vy + 1 : vy) * L - a.oy) * ivy : inf;
-    double tnz = dz != 0.0 ? ((double)(dz > 0.0 ? vz + 1 : vz) * L - a.oz) * ivz : inf;
+    DenseWalk w(a.ox, a.oy, a.oz, dx, dy, dz, a.leaf);
     double t_enter = 0.0, lo = 0.0, hi = 0.0;
     int j_hit = -1;
-    long long slot = dense_brick_find(ix, vx, vy, vz);
+    long long slot = dense_brick_find(ix, w.vx, w.vy, w.vz);
     for (int s = 0; s < DENSE_RAY_MAX_STEPS; s++) {
       if (t_enter > a.max_range) break;
-      const int ax = (tnx <= tny && tnx <= tnz) ? 0 : (tny <= tnz ? 1 : 2);
-      const double t_exit = ax == 0 ? tnx : (ax == 1 ? tny : tnz);
+      const int ax = w.axis();
+      const double t_exit = w.t_next(ax);
       if (slot >= 0 && t_exit > a.min_range) {
-        const unsigned bit = dense_local_bit(vx, vy, vz);
+        const unsigned bit = dense_local_bit(w.vx, w.vy, w.vz);
         const unsigned long long* m = ix.mask + slot * DENSE_BRICK_WORDS;
         const unsigned long long w = __ldg(&m[bit >> 6]);
         if ((w >> (bit & 63)) & 1ull) {
@@ -757,21 +797,7 @@ dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, Den
         }
       }
       t_enter = t_exit;
-      bool crossed;
-      if (ax == 0) {
-        vx += stx;
-        tnx = ((double)(stx > 0 ? vx + 1 : vx) * L - a.ox) * ivx;
-        crossed = ((vx + (1 << 20)) & 7) == (stx > 0 ? 0 : 7);
-      } else if (ax == 1) {
-        vy += sty;
-        tny = ((double)(sty > 0 ? vy + 1 : vy) * L - a.oy) * ivy;
-        crossed = ((vy + (1 << 20)) & 7) == (sty > 0 ? 0 : 7);
-      } else {
-        vz += stz;
-        tnz = ((double)(stz > 0 ? vz + 1 : vz) * L - a.oz) * ivz;
-        crossed = ((vz + (1 << 20)) & 7) == (stz > 0 ? 0 : 7);
-      }
-      if (crossed) slot = dense_brick_find(ix, vx, vy, vz);
+      if (w.step(ax)) slot = dense_brick_find(ix, w.vx, w.vy, w.vz);
     }
     if (j_hit >= 0) {  // the surfel range, outside the walk (its division stays out of the loop)
       double t = lo;
@@ -795,6 +821,134 @@ dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, Den
   }
   range[i] = __int_as_float(0x7f800000);  // no hit
   index[i] = -1;
+}
+
+// ---- carve mode of the visibility pass (include/loam_b200.h "loam_b200_dense_carving")
+// Live occupancy index: the ray index's brick hash and 512-bit masks over the live table (no base, no sorted array: it
+// stores keys and masks only, so a rehash of the voxel table leaves it valid).  Built from the table when carve mode
+// is switched on, then kept current by the insertion (dense_live_insert_kernel sets the bits of the voxels it admits);
+// it grows like the table, from a host-side bound of its bricks, with a rehash on the device.  ctr->bricks counts
+// the claimed bricks, so the host can tighten that bound from the counters each insertion mirrors.
+struct DenseLiveIndex {                // device view, by value in the kernel arguments
+  unsigned long long* key;             // brick key per slot, DENSE_EMPTY when free
+  unsigned long long* mask;            // DENSE_BRICK_WORDS words per slot
+  unsigned long long slots_mask;       // slots - 1 (a power of two, load factor <= 0.5)
+};
+
+// set voxel `key`'s bit: find or claim its brick (a claim counts a brick)
+__device__ __forceinline__ void dense_live_set(const DenseLiveIndex& ix, unsigned long long key,
+                                               DenseCounters* __restrict__ ctr) {
+  const unsigned long long c = dense_brick_composite(key), brick = c >> 9;
+  const unsigned bit = (unsigned)(c & 511);
+  unsigned long long h = dense_hash(brick) & ix.slots_mask;
+  for (;;) {
+    const unsigned long long prev = atomicCAS(&ix.key[h], DENSE_EMPTY, brick);
+    if (prev == DENSE_EMPTY) atomicAdd(&ctr->bricks, 1ull);
+    if (prev == DENSE_EMPTY || prev == brick) break;
+    h = (h + 1) & ix.slots_mask;
+  }
+  atomicOr(&ix.mask[h * DENSE_BRICK_WORDS + (bit >> 6)], 1ull << (bit & 63));
+}
+
+// build: one thread per table slot (carve mode switched on with voxels stored; never on the per-sweep path)
+__global__ void dense_live_build_kernel(const DenseSlot* __restrict__ t, unsigned long long size, DenseLiveIndex ix,
+                                        DenseCounters* __restrict__ ctr) {
+  const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
+  if (i >= size) return;
+  const unsigned long long k = t[i].key;
+  if (k != DENSE_EMPTY) dense_live_set(ix, k, ctr);
+}
+
+// growth: every brick of the old index moves to the new one with its mask (each brick once: a plain claim)
+__global__ void dense_live_rehash_kernel(const unsigned long long* __restrict__ old_key,
+                                         const unsigned long long* __restrict__ old_mask, unsigned long long old_slots,
+                                         DenseLiveIndex ix) {
+  const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
+  if (i >= old_slots) return;
+  const unsigned long long b = old_key[i];
+  if (b == DENSE_EMPTY) return;
+  unsigned long long h = dense_hash(b) & ix.slots_mask;
+  while (atomicCAS(&ix.key[h], DENSE_EMPTY, b) != DENSE_EMPTY) h = (h + 1) & ix.slots_mask;
+#pragma unroll
+  for (int w = 0; w < DENSE_BRICK_WORDS; w++) ix.mask[h * DENSE_BRICK_WORDS + w] = old_mask[i * DENSE_BRICK_WORDS + w];
+}
+
+// in the insertion, between dense_insert_kernel and dense_finish_kernel: the voxels that kernel admitted (new runs
+// ranked below the room, the same test on the same ctr->voxels) get their bits
+__global__ void dense_live_insert_kernel(DenseRuns runs, const int* __restrict__ n_runs, const unsigned* __restrict__ rank,
+                                         const unsigned* __restrict__ block_off, DenseLiveIndex ix,
+                                         DenseCounters* __restrict__ ctr, unsigned long long max_voxels) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= *n_runs || runs.slot[r] != -1) return;
+  const unsigned long long nr = rank[r] + block_off[r / SCAN_BS];
+  if (ctr->voxels + nr >= max_voxels) return;
+  dense_live_set(ix, runs.key[r], ctr);
+}
+
+// Misses of one pass without a pass over the table: stamp[s] (one word per table slot) holds 2e when slot s is in K
+// for pass e and 2e + 1 once a ray of pass e has carved it; stale words from earlier passes match neither.
+struct DenseCarveArgs {                // by value in the kernel arguments
+  double ox, oy, oz;                   // origin: the pose's float pos
+  double leaf, margin, max_range;
+  unsigned k_code, c_code;             // 2e and 2e + 1 of this pass
+};
+
+// K: one thread per point, the voxel by the map's rule (dense_key_of); a stored one is stamped "in K"
+__global__ void dense_carve_mark_kernel(const float4* __restrict__ p, int n, float inv, const DenseSlot* __restrict__ t,
+                                        unsigned long long tmask, unsigned* __restrict__ stamp, unsigned k_code) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long k = dense_key_of(p[i], inv);
+  if (k == DENSE_EMPTY) return;
+  const long long s = dense_find(t, tmask, k);
+  if (s >= 0) stamp[s] = k_code;
+}
+
+// One thread per ray (tests/carve_reference.py restates it), fp64 without FMA: e = p - o, r = sqrt((ex*ex + ey*ey) +
+// ez*ez), d = e / r (a non-finite p or r == 0 casts nothing); T = min(r - margin, max_range); DenseWalk from o along d
+// until the first voxel with t_exit > T; every voxel before it that the index holds is carved.  One brick probe per
+// brick entered, one mask word per voxel inside a non-empty brick, a table probe only for an occupied voxel.  The
+// first ray to carve a slot that is not in K moves its stamp to c_code and adds the pass's one miss, so the count
+// depends neither on the thread order nor on how many rays cross the voxel.
+__global__ void __launch_bounds__(128)
+dense_carve_kernel(const float4* __restrict__ p, int n, DenseCarveArgs a, DenseRayIndex ix, DenseSlot* t,
+                   unsigned long long tmask, unsigned* stamp) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 q = p[i];
+  if (!(isfinite(q.x) && isfinite(q.y) && isfinite(q.z))) return;
+  const double ex = (double)q.x - a.ox, ey = (double)q.y - a.oy, ez = (double)q.z - a.oz;
+  const double r = sqrt((ex * ex + ey * ey) + ez * ez);
+  if (!(r > 0.0)) return;
+  const double rm = r - a.margin;
+  const double T = rm < a.max_range ? rm : a.max_range;
+  DenseWalk w(a.ox, a.oy, a.oz, ex / r, ey / r, ez / r, a.leaf);
+  long long slot = dense_brick_find(ix, w.vx, w.vy, w.vz);
+  for (int s = 0; s < DENSE_RAY_MAX_STEPS; s++) {
+    const int ax = w.axis();
+    if (w.t_next(ax) > T) break;
+    if (slot >= 0) {
+      const unsigned bit = dense_local_bit(w.vx, w.vy, w.vz);
+      if ((__ldg(&ix.mask[slot * DENSE_BRICK_WORDS + (bit >> 6)]) >> (bit & 63)) & 1ull) {
+        constexpr int H = 1 << 20;
+        const unsigned long long key = ((unsigned long long)(w.vz + H) << 42) |
+                                       ((unsigned long long)(w.vy + H) << 21) | (unsigned long long)(w.vx + H);
+        const long long ts = dense_find(t, tmask, key);
+        if (ts >= 0) {
+          unsigned old = stamp[ts];
+          while (old != a.k_code && old != a.c_code) {
+            const unsigned prev = atomicCAS(&stamp[ts], old, a.c_code);
+            if (prev == old) {
+              t[ts].evidence = dense_add_miss(t[ts].evidence);
+              break;
+            }
+            old = prev;
+          }
+        }
+      }
+    }
+    if (w.step(ax)) slot = dense_brick_find(ix, w.vx, w.vy, w.vz);
+  }
 }
 
 // Host-side state of the map (loam_b200_ctx::dense).  The insertion runs on its own stream with its own sort scratch,
@@ -822,6 +976,14 @@ struct DenseMap {
   double vis_h_res = 0.0, vis_v_res = 0.0, vis_margin = 0.0;  // visibility pass (vis_h_res == 0: off)
   int vis_rows = 0, vis_cols = 0;
   DevBuf<unsigned> image;         // range image of the sweep being observed (float bits, DENSE_NO_RETURN when empty)
+  double carve_margin = 0.0, carve_max = 0.0;  // carve mode (carve_max == 0: off)
+  unsigned long long* live_key = nullptr;      // carve mode's occupancy index (stream-ordered allocations on `stream`)
+  unsigned long long* live_mask = nullptr;
+  unsigned long long live_slots = 0;           // 0: no index (carve mode off, or dropped by a clear)
+  unsigned long long live_bound = 0;           // upper bound of its bricks, known without a readback
+  unsigned* stamp = nullptr;                   // carve mode's per-slot stamps (table_size words once allocated)
+  unsigned long long stamp_size = 0;
+  unsigned epoch = 0;                          // the last carve pass (stamps 2e / 2e + 1)
   DevBuf<DenseCounters> ctr;
   PinBuf<DenseCounters> ctr_host;
   DenseSlot* table = nullptr;     // stream-ordered allocation (cudaMallocAsync on `stream`)
@@ -833,12 +995,19 @@ struct DenseMap {
     if (stream) {
       cudaStreamSynchronize(stream);
       if (table) cudaFreeAsync(table, stream);
+      if (live_key) cudaFreeAsync(live_key, stream);
+      if (live_mask) cudaFreeAsync(live_mask, stream);
+      if (stamp) cudaFreeAsync(stamp, stream);
       cudaStreamSynchronize(stream);
       cudaStreamDestroy(stream);
     }
     stream = nullptr;
     table = nullptr;
     table_size = 0;
+    live_key = live_mask = nullptr;
+    live_slots = live_bound = 0;
+    stamp = nullptr;
+    stamp_size = 0;
     sort.keys_a.release(); sort.keys_b.release(); sort.vals_a.release(); sort.vals_b.release(); sort.hist.release();
     keys64.release(); skeys.release(); pos.release(); rank.release(); run_key.release(); run_count.release();
     run_sum.release(); run_slot.release(); slots.release(); ints.release(); out.release(); out_count.release();

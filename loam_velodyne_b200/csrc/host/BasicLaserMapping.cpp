@@ -116,6 +116,10 @@ void BasicLaserMapping::enableDenseVisibility(double hRes, double vRes, double m
   _gpu->check(loam_b200_dense_visibility(_gpu->get(), hRes, vRes, margin), "loam_b200_dense_visibility");
 }
 
+void BasicLaserMapping::enableDenseCarving(double margin, double maxRange) {
+  _gpu->check(loam_b200_dense_carving(_gpu->get(), margin, maxRange), "loam_b200_dense_carving");
+}
+
 void BasicLaserMapping::denseMapFiltered(Cloud& out, double maxMissRatio, std::vector<uint32_t>* counts,
                                          std::vector<uint16_t>* hits, std::vector<uint16_t>* misses) {
   const int n = (int)denseMapStats().voxels;  // the voxels kept are a subset

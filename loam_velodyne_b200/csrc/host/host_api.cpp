@@ -542,6 +542,10 @@ int loam_b200_map_dense_visibility(void* h, double h_res_deg, double v_res_deg, 
   if (const int rc = map_in_flight((MapH*)h)) return rc;
   return guarded([&] { ((MapH*)h)->m.enableDenseVisibility(h_res_deg, v_res_deg, margin); return 0; });
 }
+int loam_b200_map_dense_carving(void* h, double margin, double max_range) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  return guarded([&] { ((MapH*)h)->m.enableDenseCarving(margin, max_range); return 0; });
+}
 int loam_b200_map_dense_export_filtered(void* h, double max_miss_ratio, float* xyzi, unsigned int* counts,
                                         unsigned short* hits, unsigned short* misses, int cap, int* n_out) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;

@@ -125,6 +125,11 @@ class BasicLaserMapping {
   // optimised pose and counts a miss for every stored voxel that lies more than `margin` metres in front of the return
   // in its pixel.  hRes = 0 turns it off; throws without the dense map and on bad arguments.
   void enableDenseVisibility(double hRes, double vRes, double margin);
+  // Carve mode of that pass (off by default; include/loam_b200.h "loam_b200_dense_carving"): every process() walks each
+  // registered point's ray from the optimised pose through the map and counts one miss for every stored voxel a ray
+  // crosses more than `margin` metres short of its return (up to maxRange) that no point of the sweep falls into.
+  // maxRange = 0 turns it off; throws without the dense map, on bad arguments and while the range-image mode is on.
+  void enableDenseCarving(double margin, double maxRange);
   // the voxels with misses <= maxMissRatio * hits (a voxel's hits: the sweeps that put points into it); +inf returns
   // every voxel, as denseMap above.  hits / misses: per-voxel evidence counters (saturating at 65535) when non-null.
   void denseMapFiltered(pcl::PointCloud<pcl::PointXYZI>& out, double maxMissRatio,

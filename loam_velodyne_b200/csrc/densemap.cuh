@@ -3,9 +3,9 @@
 // the whole run, which the reference itself never keeps (its cube grid forgets cubes that roll out of the window).
 //
 // Voxel of a point: v_a = (int)floorf(c_a * (1.0f / leaf)) per axis, PCL VoxelGrid's index before it subtracts min_b
-// (voxel.cuh: voxel_key_of), so one cloud's voxels form the same partition as VoxelGrid.  Key = (v_z + 2^20) << 42 |
-// (v_y + 2^20) << 21 | (v_x + 2^20): z-major, so ascending keys are VoxelGrid's output order.  Points that are not
-// finite or whose voxel lies outside [-2^20, 2^20) on an axis are skipped (and counted).
+// (voxel.cuh: voxel_key_of), so one cloud's voxels form the same partition as VoxelGrid.  Its key is given by the key
+// codec below: z-major, so ascending keys are VoxelGrid's output order.  Points that are not finite or whose voxel lies
+// outside [-2^20, 2^20) on an axis are skipped (and counted).
 //
 // One insert of n points:
 //   key kernel -> stable two-pass LSD sort of the 64-bit keys (low word, then high word; radix_sort_pairs) -> run heads
@@ -23,6 +23,8 @@
 // an entry.  Keys are unique within one insert, so no value update needs an atomic.
 #pragma once
 
+#include <cmath>
+
 #include "linalg.cuh"
 #include "mapping_lm.cuh"
 #include "voxel.cuh"
@@ -30,7 +32,44 @@
 namespace loamb {
 
 constexpr unsigned long long DENSE_EMPTY = ~0ull;  // empty table slot; also the key of a skipped point (sorts last)
-constexpr float DENSE_KEY_LIM = 1048576.f;          // 2^20 voxels per half axis
+
+// ---- voxel key codec: the only statement of the key layout.  Voxel (v_x, v_y, v_z) has the biased indices
+// u_a = v_a + 2^20 in [0, 2^21) and the key u_z << 42 | u_y << 21 | u_x.  Its 8^3 brick has the key
+// (u_z >> 3) << 36 | (u_y >> 3) << 18 | (u_x >> 3), and its bit in the brick's 512-bit mask is
+// (u_z & 7) << 6 | (u_y & 7) << 3 | (u_x & 7).
+constexpr int DENSE_KEY_BIAS = 1 << 20;                 // voxels per half axis
+constexpr int DENSE_AXIS = 2 * DENSE_KEY_BIAS;          // biased indices per axis
+constexpr unsigned long long DENSE_AXIS_MASK = DENSE_AXIS - 1;
+constexpr float DENSE_KEY_LIM = (float)DENSE_KEY_BIAS;
+
+__device__ __forceinline__ unsigned long long dense_pack(unsigned ux, unsigned uy, unsigned uz) {
+  return ((unsigned long long)uz << 42) | ((unsigned long long)uy << 21) | (unsigned long long)ux;
+}
+
+// key of voxel (vx, vy, vz), each inside [-2^20, 2^20)
+__device__ __forceinline__ unsigned long long dense_key(int vx, int vy, int vz) {
+  return dense_pack((unsigned)(vx + DENSE_KEY_BIAS), (unsigned)(vy + DENSE_KEY_BIAS), (unsigned)(vz + DENSE_KEY_BIAS));
+}
+
+__device__ __forceinline__ void dense_unpack(unsigned long long key, int& ux, int& uy, int& uz) {
+  ux = (int)(key & DENSE_AXIS_MASK);
+  uy = (int)((key >> 21) & DENSE_AXIS_MASK);
+  uz = (int)(key >> 42);
+}
+
+__device__ __forceinline__ unsigned long long dense_brick(int ux, int uy, int uz) {
+  return ((unsigned long long)(uz >> 3) << 36) | ((unsigned long long)(uy >> 3) << 18) | (unsigned long long)(ux >> 3);
+}
+
+__device__ __forceinline__ unsigned dense_brick_bit(int ux, int uy, int uz) {
+  return ((unsigned)(uz & 7) << 6) | ((unsigned)(uy & 7) << 3) | (unsigned)(ux & 7);
+}
+
+// host: the voxel floor(o / leaf) of coordinate o lies inside the key range (NaN and +-inf do not)
+inline bool dense_in_key_range(double o, double leaf) {
+  const double v = std::floor(o / leaf);
+  return v >= -(double)DENSE_KEY_BIAS && v < (double)DENSE_KEY_BIAS;
+}
 
 struct __align__(16) DenseSlot {  // 48 B
   unsigned long long key;
@@ -63,10 +102,7 @@ __device__ __forceinline__ unsigned long long dense_key_of(const float4& q, floa
   if (!(fx >= -DENSE_KEY_LIM && fx < DENSE_KEY_LIM && fy >= -DENSE_KEY_LIM && fy < DENSE_KEY_LIM &&
         fz >= -DENSE_KEY_LIM && fz < DENSE_KEY_LIM))
     return DENSE_EMPTY;
-  const unsigned long long vx = (unsigned long long)((int)fx + (1 << 20));
-  const unsigned long long vy = (unsigned long long)((int)fy + (1 << 20));
-  const unsigned long long vz = (unsigned long long)((int)fz + (1 << 20));
-  return (vz << 42) | (vy << 21) | vx;
+  return dense_key((int)fx, (int)fy, (int)fz);
 }
 
 // 64-bit finaliser of splitmix64: consecutive voxel keys spread over the whole table
@@ -281,9 +317,6 @@ __global__ void dense_centroid_kernel(const DenseSlot* __restrict__ t, const int
 }
 
 // ---- normals of the exported cloud (include/loam_b200.h "loam_b200_dense_export_normals")
-constexpr int DENSE_AXIS = 1 << 21;  // voxel indices per axis in the key (v + 2^20 in [0, 2^21))
-constexpr unsigned long long DENSE_AXIS_MASK = DENSE_AXIS - 1;
-
 // first position in [lo, hi) of the ascending keys whose key is >= `key`
 __device__ __forceinline__ int dense_lower_bound(const unsigned long long* __restrict__ k, int lo, int hi,
                                                  unsigned long long key) {
@@ -295,25 +328,16 @@ __device__ __forceinline__ int dense_lower_bound(const unsigned long long* __res
   return lo;
 }
 
-// One thread per exported voxel, over the export's own arrays (keys ascending, centroids in the same order), so the
-// miss-ratio filter is already applied and the table is never touched.  Neighbours: the exported voxels within `radius`
-// voxels on every axis, visited in ascending key order -- per (z, y) row inside the key range, a lower bound of the
-// row's first key (x clamped to the range), then forward while the key stays in the row.  Rows outside the range are
-// skipped, so an offset never wraps into the next row or plane.  Centred fp64 sums of the fp32 centroids, covariance
-// rounded to fp32 once per entry, sym_eigen<3>, curvature ev0 / (ev0 + ev1 + ev2), normal flipped towards the viewpoint.
-// Fewer than 3 neighbours, or no convergence: NaN normal and curvature.  The library is built without FMA contraction,
-// so every product and sum rounds on its own, as in tests/normals_reference.py.
-__global__ void __launch_bounds__(128)
-dense_normals_kernel(const unsigned long long* __restrict__ skey, const float4* __restrict__ cent, int n, int radius,
-                     double3 vp, float4* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const unsigned long long key = skey[i];
-  const int vx = (int)(key & DENSE_AXIS_MASK), vy = (int)((key >> 21) & DENSE_AXIS_MASK), vz = (int)(key >> 42);
-  const float4 cv = cent[i];
-  const double cx = (double)cv.x, cy = (double)cv.y, cz = (double)cv.z;
-  double s1x = 0.0, s1y = 0.0, s1z = 0.0, sxx = 0.0, sxy = 0.0, sxz = 0.0, syy = 0.0, syz = 0.0, szz = 0.0;
-  int k = 0;
+// Calls visit(j) for every position j in [0, n) of the ascending keys skey whose voxel lies within `radius` voxels of
+// `key`'s on every axis, in ascending key order: per (z, y) row inside the key range, a lower bound of the row's first
+// key (x clamped to the range), then forward while the key stays in the row.  Rows outside the range are skipped, so an
+// offset never wraps into the next row or plane.  The order is load-bearing: it fixes the fp64 sums of the normals and
+// the first-smallest tie rule of the alignment's match.
+template <typename F>
+__device__ __forceinline__ void dense_box_walk(const unsigned long long* __restrict__ skey, int n, unsigned long long key,
+                                               int radius, F&& visit) {
+  int vx, vy, vz;
+  dense_unpack(key, vx, vy, vz);
   const unsigned long long x0 = (unsigned long long)max(vx - radius, 0);
   const unsigned long long x1 = (unsigned long long)min(vx + radius, DENSE_AXIS - 1);
   int lo = 0;  // rows ascend in key order: each row's search starts where the previous row ended
@@ -321,26 +345,45 @@ dense_normals_kernel(const unsigned long long* __restrict__ skey, const float4* 
     if (z < 0 || z >= DENSE_AXIS) continue;
     for (int y = vy - radius; y <= vy + radius; y++) {
       if (y < 0 || y >= DENSE_AXIS) continue;
-      const unsigned long long row = ((unsigned long long)z << 42) | ((unsigned long long)y << 21);
+      const unsigned long long row = dense_pack(0u, (unsigned)y, (unsigned)z);
       const unsigned long long last = row | x1;
       int j = dense_lower_bound(skey, lo, n, row | x0);
-      for (; j < n && skey[j] <= last; j++) {
-        const float4 cw = cent[j];
-        const double dx = (double)cw.x - cx, dy = (double)cw.y - cy, dz = (double)cw.z - cz;
-        s1x += dx;
-        s1y += dy;
-        s1z += dz;
-        sxx += dx * dx;
-        sxy += dx * dy;
-        sxz += dx * dz;
-        syy += dy * dy;
-        syz += dy * dz;
-        szz += dz * dz;
-        k++;
-      }
+      for (; j < n && skey[j] <= last; j++) visit(j);
       lo = j;
     }
   }
+}
+
+// One thread per exported voxel, over the export's own arrays (keys ascending, centroids in the same order), so the
+// miss-ratio filter is already applied and the table is never touched.  Neighbours: the exported voxels of
+// dense_box_walk.  Centred fp64 sums of the fp32 centroids, covariance rounded to fp32 once per entry, sym_eigen<3>,
+// curvature ev0 / (ev0 + ev1 + ev2), normal flipped towards the viewpoint.  Fewer than 3 neighbours, or no
+// convergence: NaN normal and curvature.  The library is built without FMA contraction, so every product and sum
+// rounds on its own, as in tests/normals_reference.py.
+__global__ void __launch_bounds__(128)
+dense_normals_kernel(const unsigned long long* __restrict__ skey, const float4* __restrict__ cent, int n, int radius,
+                     double3 vp, float4* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long key = skey[i];
+  const float4 cv = cent[i];
+  const double cx = (double)cv.x, cy = (double)cv.y, cz = (double)cv.z;
+  double s1x = 0.0, s1y = 0.0, s1z = 0.0, sxx = 0.0, sxy = 0.0, sxz = 0.0, syy = 0.0, syz = 0.0, szz = 0.0;
+  int k = 0;
+  dense_box_walk(skey, n, key, radius, [&](int j) {
+    const float4 cw = cent[j];
+    const double dx = (double)cw.x - cx, dy = (double)cw.y - cy, dz = (double)cw.z - cz;
+    s1x += dx;
+    s1y += dy;
+    s1z += dz;
+    sxx += dx * dx;
+    sxy += dx * dy;
+    sxz += dx * dz;
+    syy += dy * dy;
+    syz += dy * dz;
+    szz += dz * dz;
+    k++;
+  });
   const float qnan = __int_as_float(0x7fc00000);
   if (k < 3) {
     out[i] = make_float4(qnan, qnan, qnan, qnan);
@@ -391,9 +434,7 @@ __global__ void dense_target_gather_kernel(const unsigned long long* __restrict_
 
 // One Gauss-Newton iteration of a cloud against the target, one thread per point (point i in CTA i / LM_THREADS):
 //   q = associate_to_map(pose, p); v = voxel of q (dense_key_of with the target's leaf);
-//   candidates: the target voxels within `radius` of v on every axis whose normal_x is not NaN, visited in ascending key
-//   order by the row walk of dense_normals_kernel (rows outside the key range are skipped and never wrap); the first
-//   smallest d2 = (dx*dx + dy*dy) + dz*dz, d = c - q, wins when d2 < gate;
+//   candidates: the target voxels of dense_box_walk around v whose normal_x is not NaN; the first smallest d2 = (dx*dx + dy*dy) + dz*dz, d = c - q, wins when d2 < gate;
 //   pd2 = (nx*(qx - cx) + ny*(qy - cy)) + nz*(qz - cz); s = 1 - 0.9f*|pd2| / sqrtf(sqrtf(|p|^2)) with the SENSOR-frame p;
 //   selected when (double)s > 0.1; coeff = s * (n, pd2); Jacobian row and rhs of the scan-to-map kernels.
 // Slots 0..26 of the 32 sums: AtA (upper triangle) and AtB; 27: selected rows; 28: sum of pd2^2 over them.  The
@@ -491,31 +532,17 @@ dense_align_kernel(const unsigned long long* __restrict__ skey, const float4* __
       associate_to_map(a, po, qx, qy, qz);
       const unsigned long long key = dense_key_of(make_float4(qx, qy, qz, 0.f), inv);
       if (key != DENSE_EMPTY) {
-        const int vx = (int)(key & DENSE_AXIS_MASK), vy = (int)((key >> 21) & DENSE_AXIS_MASK), vz = (int)(key >> 42);
-        const unsigned long long x0 = (unsigned long long)max(vx - radius, 0);
-        const unsigned long long x1 = (unsigned long long)min(vx + radius, DENSE_AXIS - 1);
         float best_d2 = gate;  // strict < from the gate: the first smallest d2 below it
-        int lo = 0;            // rows ascend in key order: each row's search starts where the previous row ended
-        for (int z = vz - radius; z <= vz + radius; z++) {
-          if (z < 0 || z >= DENSE_AXIS) continue;
-          for (int y = vy - radius; y <= vy + radius; y++) {
-            if (y < 0 || y >= DENSE_AXIS) continue;
-            const unsigned long long row = ((unsigned long long)z << 42) | ((unsigned long long)y << 21);
-            const unsigned long long last = row | x1;
-            int j = dense_lower_bound(skey, lo, m, row | x0);
-            for (; j < m && skey[j] <= last; j++) {
-              if (isnan(nrm[j].x)) continue;
-              const float4 c = cent[j];
-              const float dx = c.x - qx, dy = c.y - qy, dz = c.z - qz;
-              const float d2 = (dx * dx + dy * dy) + dz * dz;
-              if (d2 < best_d2) {
-                best_d2 = d2;
-                best = j;
-              }
-            }
-            lo = j;
+        dense_box_walk(skey, m, key, radius, [&](int j) {
+          if (isnan(nrm[j].x)) return;
+          const float4 c = cent[j];
+          const float dx = c.x - qx, dy = c.y - qy, dz = c.z - qz;
+          const float d2 = (dx * dx + dy * dy) + dz * dz;
+          if (d2 < best_d2) {
+            best_d2 = d2;
+            best = j;
           }
-        }
+        });
       }
       if (best >= 0) {
         const float4 c = cent[best], nv = nrm[best];
@@ -620,22 +647,56 @@ __global__ void dense_visibility_kernel(DenseSlot* t, unsigned long long size, D
   }
 }
 
-// ---- ray casting the target (include/loam_b200.h "loam_b200_dense_raycast")
-// Ray index: a hash table of 8^3-voxel bricks.  A brick's key is the voxel key >> 3 per axis (bz << 36 | by << 18 | bx);
-// its voxel's local bit is (lz << 6 | ly << 3 | lx).  Built from the target's keys: composite key brick << 9 | bit,
-// sorted (dense_sort64), so each brick's voxels are one run in local-bit order; idx[j] = the target index of sorted
-// position j, and a brick's slot keeps its 512-bit mask and the position of its run's head.  A voxel's target index
-// is then idx[base + popc(mask below its bit)].
+// ---- 8^3-brick index: carve mode's live occupancy index and the target's ray index
+// An open-addressing hash of brick keys (dense_hash, linear probe, load factor <= 0.5) with each brick's 512-bit mask
+// of occupied voxels; brick key and bit come from the key codec.  The ray index also keeps, per slot, the sorted
+// position of its brick's first voxel (base) and, per sorted position, a target index (idx); the live index has neither.
 constexpr int DENSE_BRICK_WORDS = 8;                 // 64-bit words of a brick's mask
-constexpr int DENSE_RAY_MAX_STEPS = 3 * 65536 + 4;   // max_range / leaf <= 65536 crosses at most sqrt(3) 65536 + 3 faces
 
-struct DenseRayIndex {                 // device view, by value in the kernel arguments
-  const unsigned long long* key;       // brick key per slot, DENSE_EMPTY when free
-  const unsigned long long* mask;      // DENSE_BRICK_WORDS words per slot
-  const unsigned* base;                // per slot: sorted position of the brick's first voxel
-  const int* idx;                      // per sorted position: target index
-  unsigned long long slots_mask;       // slots - 1 (a power of two)
+struct DenseBrickIndex {                    // device view, by value in the kernel arguments
+  unsigned long long* key = nullptr;        // brick key per slot, DENSE_EMPTY when free; null: no index
+  unsigned long long* mask = nullptr;       // DENSE_BRICK_WORDS words per slot
+  unsigned long long slots_mask = 0;        // slots - 1 (a power of two)
+  unsigned* base = nullptr;                 // ray index: per slot, sorted position of the brick's first voxel
+  int* idx = nullptr;                       // ray index: per sorted position, target index
+
+  __host__ __device__ unsigned long long slots() const { return key ? slots_mask + 1 : 0; }
+
+  // the slot of `brick`; when absent, -1 (find) or a slot claimed for it, with *claimed set (find_or_claim)
+  template <bool CLAIM>
+  __device__ __forceinline__ long long probe(unsigned long long brick, bool* claimed) const {
+    unsigned long long h = dense_hash(brick) & slots_mask;
+    for (;;) {
+      const unsigned long long k = CLAIM ? atomicCAS(&key[h], DENSE_EMPTY, brick) : __ldg(&key[h]);
+      if (k == brick) return (long long)h;
+      if (k == DENSE_EMPTY) {
+        if (!CLAIM) return -1;
+        if (claimed) *claimed = true;
+        return (long long)h;
+      }
+      h = (h + 1) & slots_mask;
+    }
+  }
+  __device__ __forceinline__ long long find(unsigned long long brick) const { return probe<false>(brick, nullptr); }
+  __device__ __forceinline__ long long find_or_claim(unsigned long long b, bool* claimed = nullptr) const {
+    return probe<true>(b, claimed);
+  }
+  __device__ __forceinline__ void set(long long slot, unsigned bit) const {
+    atomicOr(&mask[slot * DENSE_BRICK_WORDS + (bit >> 6)], 1ull << (bit & 63));
+  }
+  __device__ __forceinline__ unsigned long long word(long long slot, unsigned bit) const {
+    return __ldg(&mask[slot * DENSE_BRICK_WORDS + (bit >> 6)]);
+  }
+  __device__ __forceinline__ bool test(long long slot, unsigned bit) const {
+    return (word(slot, bit) >> (bit & 63)) & 1ull;
+  }
 };
+
+// ---- ray casting the target (include/loam_b200.h "loam_b200_dense_raycast")
+// Ray index: built from the target's keys: composite key brick << 9 | bit, sorted (dense_sort64), so each brick's
+// voxels are one run in bit order; idx[j] = the target index of sorted position j, and a brick's slot keeps its mask
+// and the position of its run's head.  A voxel's target index is then idx[base + popc(mask below its bit)].
+constexpr int DENSE_RAY_MAX_STEPS = 3 * 65536 + 4;   // max_range / leaf <= 65536 crosses at most sqrt(3) 65536 + 3 faces
 
 struct DenseRayArgs {                  // by value in the kernel arguments
   double ox, oy, oz;                   // origin: the pose's float pos
@@ -644,9 +705,9 @@ struct DenseRayArgs {                  // by value in the kernel arguments
 };
 
 __device__ __forceinline__ unsigned long long dense_brick_composite(unsigned long long key) {
-  const unsigned long long vx = key & DENSE_AXIS_MASK, vy = (key >> 21) & DENSE_AXIS_MASK, vz = key >> 42;
-  const unsigned long long brick = ((vz >> 3) << 36) | ((vy >> 3) << 18) | (vx >> 3);
-  return (brick << 9) | ((vz & 7) << 6) | ((vy & 7) << 3) | (vx & 7);
+  int ux, uy, uz;
+  dense_unpack(key, ux, uy, uz);
+  return (dense_brick(ux, uy, uz) << 9) | dense_brick_bit(ux, uy, uz);
 }
 
 // composite keys of the target's voxels + the (low word, index) pairs of the first sort pass
@@ -671,54 +732,29 @@ __global__ void dense_brick_count_kernel(const unsigned long long* __restrict__ 
   if (j == 0 || (comp[o] >> 9) != (comp[order[j - 1]] >> 9)) atomicAdd(bricks, 1);
 }
 
-// per sorted position: find or claim the brick's slot (load factor <= 0.5), set the voxel's bit; the head sets base
-__global__ void dense_brick_fill_kernel(const unsigned long long* __restrict__ comp, const int* __restrict__ idx, int n,
-                                        unsigned long long* bkey, unsigned long long* bmask, unsigned* __restrict__ bbase,
-                                        unsigned long long smask) {
+// per sorted position: find or claim the brick's slot, set the voxel's bit; the head sets base
+__global__ void dense_brick_fill_kernel(const unsigned long long* __restrict__ comp, int n, DenseBrickIndex ix) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
-  const unsigned long long c = comp[idx[j]], brick = c >> 9;
-  const unsigned bit = (unsigned)(c & 511);
-  unsigned long long h = dense_hash(brick) & smask;
-  for (;;) {
-    const unsigned long long prev = atomicCAS(&bkey[h], DENSE_EMPTY, brick);
-    if (prev == DENSE_EMPTY || prev == brick) break;
-    h = (h + 1) & smask;
-  }
-  atomicOr(&bmask[h * DENSE_BRICK_WORDS + (bit >> 6)], 1ull << (bit & 63));
-  if (j == 0 || (comp[idx[j - 1]] >> 9) != brick) bbase[h] = (unsigned)j;
+  const unsigned long long c = comp[ix.idx[j]], brick = c >> 9;
+  const long long h = ix.find_or_claim(brick);
+  ix.set(h, (unsigned)(c & 511));
+  if (j == 0 || (comp[ix.idx[j - 1]] >> 9) != brick) ix.base[h] = (unsigned)j;
 }
 
-// slot of the brick holding voxel (vx, vy, vz), -1 when the brick is empty or the voxel outside the key range
-__device__ __forceinline__ long long dense_brick_find(const DenseRayIndex& ix, int vx, int vy, int vz) {
-  constexpr int H = 1 << 20;
-  if (vx < -H || vx >= H || vy < -H || vy >= H || vz < -H || vz >= H) return -1;
-  const unsigned long long brick = ((unsigned long long)((vz + H) >> 3) << 36) |
-                                   ((unsigned long long)((vy + H) >> 3) << 18) | (unsigned long long)((vx + H) >> 3);
-  unsigned long long h = dense_hash(brick) & ix.slots_mask;
-  for (;;) {
-    const unsigned long long k = __ldg(&ix.key[h]);
-    if (k == brick) return (long long)h;
-    if (k == DENSE_EMPTY) return -1;
-    h = (h + 1) & ix.slots_mask;
-  }
-}
-
-__device__ __forceinline__ unsigned dense_local_bit(int vx, int vy, int vz) {
-  constexpr int H = 1 << 20;
-  return ((unsigned)((vz + H) & 7) << 6) | ((unsigned)((vy + H) & 7) << 3) | (unsigned)((vx + H) & 7);
-}
-
-// The voxel walk of a ray from o along d (Amanatides-Woo), shared by the ray cast and carve mode, fp64 without FMA:
-// start voxel floor(o_a / L); per axis with d_a != 0 inv_a = 1 / d_a and t_next_a = ((double)k * L - o_a) * inv_a with
-// k = v_a + 1 (d_a > 0) or v_a (d_a < 0); +inf when d_a == 0.  The current voxel spans [t_enter, t_exit = min t_next);
-// step() moves along axis() -- the smallest t_next, ties x, y, z -- and recomputes only that axis's t_next, from its new
-// index, so no error accumulates.  It returns whether the step entered another 8^3 brick.
+// The voxel walk of a ray from o along d (Amanatides-Woo) through a brick index, shared by the ray cast and carve mode,
+// fp64 without FMA: start voxel floor(o_a / L); per axis with d_a != 0 inv_a = 1 / d_a and t_next_a = ((double)k * L -
+// o_a) * inv_a with k = v_a + 1 (d_a > 0) or v_a (d_a < 0); +inf when d_a == 0.  The current voxel spans [t_enter,
+// t_exit = min t_next); step() moves along axis() -- the smallest t_next, ties x, y, z -- and recomputes only that
+// axis's t_next, from its new index, so no error accumulates.  The walk keeps `slot`, the current voxel's brick in the
+// index it walks: probed at the start and again only when a step enters another 8^3 brick.
 struct DenseWalk {
   double ox, oy, oz, L, ivx, ivy, ivz, tnx, tny, tnz;
   int vx, vy, vz, stx, sty, stz;
+  long long slot;  // -1 when the brick is empty or the voxel outside the key range
 
-  __device__ __forceinline__ DenseWalk(double ox_, double oy_, double oz_, double dx, double dy, double dz, double L_)
+  __device__ __forceinline__ DenseWalk(const DenseBrickIndex& ix, double ox_, double oy_, double oz_, double dx,
+                                       double dy, double dz, double L_)
       : ox(ox_), oy(oy_), oz(oz_), L(L_) {
     const double inf = __longlong_as_double(0x7ff0000000000000ll);
     vx = (int)floor(ox / L);
@@ -733,23 +769,40 @@ struct DenseWalk {
     tnx = dx != 0.0 ? ((double)(dx > 0.0 ? vx + 1 : vx) * L - ox) * ivx : inf;
     tny = dy != 0.0 ? ((double)(dy > 0.0 ? vy + 1 : vy) * L - oy) * ivy : inf;
     tnz = dz != 0.0 ? ((double)(dz > 0.0 ? vz + 1 : vz) * L - oz) * ivz : inf;
+    slot = brick(ix);
   }
   __device__ __forceinline__ int axis() const { return (tnx <= tny && tnx <= tnz) ? 0 : (tny <= tnz ? 1 : 2); }
   __device__ __forceinline__ double t_next(int ax) const { return ax == 0 ? tnx : (ax == 1 ? tny : tnz); }
-  __device__ __forceinline__ bool step(int ax) {
+  __device__ __forceinline__ void step(const DenseBrickIndex& ix, int ax) {
+    if (advance(ax)) slot = brick(ix);
+  }
+  // the current voxel's bit in its brick
+  __device__ __forceinline__ unsigned bit() const {
+    return dense_brick_bit(vx + DENSE_KEY_BIAS, vy + DENSE_KEY_BIAS, vz + DENSE_KEY_BIAS);
+  }
+
+ private:
+  // one step along `ax`: whether it entered another brick
+  __device__ __forceinline__ bool advance(int ax) {
     if (ax == 0) {
       vx += stx;
       tnx = ((double)(stx > 0 ? vx + 1 : vx) * L - ox) * ivx;
-      return ((vx + (1 << 20)) & 7) == (stx > 0 ? 0 : 7);
+      return ((vx + DENSE_KEY_BIAS) & 7) == (stx > 0 ? 0 : 7);
     }
     if (ax == 1) {
       vy += sty;
       tny = ((double)(sty > 0 ? vy + 1 : vy) * L - oy) * ivy;
-      return ((vy + (1 << 20)) & 7) == (sty > 0 ? 0 : 7);
+      return ((vy + DENSE_KEY_BIAS) & 7) == (sty > 0 ? 0 : 7);
     }
     vz += stz;
     tnz = ((double)(stz > 0 ? vz + 1 : vz) * L - oz) * ivz;
-    return ((vz + (1 << 20)) & 7) == (stz > 0 ? 0 : 7);
+    return ((vz + DENSE_KEY_BIAS) & 7) == (stz > 0 ? 0 : 7);
+  }
+  __device__ __forceinline__ long long brick(const DenseBrickIndex& ix) const {
+    if (vx < -DENSE_KEY_BIAS || vx >= DENSE_KEY_BIAS || vy < -DENSE_KEY_BIAS || vy >= DENSE_KEY_BIAS ||
+        vz < -DENSE_KEY_BIAS || vz >= DENSE_KEY_BIAS)
+      return -1;
+    return ix.find(dense_brick(vx + DENSE_KEY_BIAS, vy + DENSE_KEY_BIAS, vz + DENSE_KEY_BIAS));
   }
 };
 
@@ -760,9 +813,8 @@ struct DenseWalk {
 //   t_exit > min_range is the hit, at t = clamp(num / den, lo, hi) on its surfel (den != 0) or lo (no normal, or
 //   den == 0), lo = max(t_enter, min_range), hi = t_exit; t > max_range is no hit.  Then one step along the axis of the
 //   smallest t_next (ties x, y, z); t_enter = its old t_next; only its t_next is recomputed, from the new index.
-// The mask word is read per voxel only inside a non-empty brick; the hash is probed once per brick entered.
 __global__ void
-dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, DenseRayIndex ix,
+dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, DenseBrickIndex ix,
                      const float4* __restrict__ cent, const float4* __restrict__ nrm, float* __restrict__ range,
                      int* __restrict__ index) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -775,29 +827,27 @@ dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, Den
     const double x1 = a.cz * ux - a.sz * uy, y1 = a.sz * ux + a.cz * uy;
     const double y2 = a.cx * y1 - a.sx * uz, z2 = a.sx * y1 + a.cx * uz;
     const double dx = a.cy * x1 + a.sy * z2, dy = y2, dz = a.cy * z2 - a.sy * x1;
-    DenseWalk w(a.ox, a.oy, a.oz, dx, dy, dz, a.leaf);
+    DenseWalk w(ix, a.ox, a.oy, a.oz, dx, dy, dz, a.leaf);
     double t_enter = 0.0, lo = 0.0, hi = 0.0;
     int j_hit = -1;
-    long long slot = dense_brick_find(ix, w.vx, w.vy, w.vz);
     for (int s = 0; s < DENSE_RAY_MAX_STEPS; s++) {
       if (t_enter > a.max_range) break;
       const int ax = w.axis();
       const double t_exit = w.t_next(ax);
-      if (slot >= 0 && t_exit > a.min_range) {
-        const unsigned bit = dense_local_bit(w.vx, w.vy, w.vz);
-        const unsigned long long* m = ix.mask + slot * DENSE_BRICK_WORDS;
-        const unsigned long long w = __ldg(&m[bit >> 6]);
-        if ((w >> (bit & 63)) & 1ull) {
-          int below = __popcll(w & ((1ull << (bit & 63)) - 1ull));
+      if (w.slot >= 0 && t_exit > a.min_range) {
+        const unsigned bit = w.bit();
+        if (ix.test(w.slot, bit)) {  // its target index: the brick's voxels below it, after the brick's base
+          const unsigned long long* m = ix.mask + w.slot * DENSE_BRICK_WORDS;
+          int below = __popcll(ix.word(w.slot, bit) & ((1ull << (bit & 63)) - 1ull));
           for (unsigned k = 0; k < (bit >> 6); k++) below += __popcll(__ldg(&m[k]));
-          j_hit = __ldg(&ix.idx[__ldg(&ix.base[slot]) + below]);
+          j_hit = __ldg(&ix.idx[__ldg(&ix.base[w.slot]) + below]);
           lo = t_enter > a.min_range ? t_enter : a.min_range;
           hi = t_exit;
           break;
         }
       }
       t_enter = t_exit;
-      if (w.step(ax)) slot = dense_brick_find(ix, w.vx, w.vy, w.vz);
+      w.step(ix, ax);
     }
     if (j_hit >= 0) {  // the surfel range, outside the walk (its division stays out of the loop)
       double t = lo;
@@ -824,34 +874,24 @@ dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, Den
 }
 
 // ---- carve mode of the visibility pass (include/loam_b200.h "loam_b200_dense_carving")
-// Live occupancy index: the ray index's brick hash and 512-bit masks over the live table (no base, no sorted array: it
-// stores keys and masks only, so a rehash of the voxel table leaves it valid).  Built from the table when carve mode
-// is switched on, then kept current by the insertion (dense_live_insert_kernel sets the bits of the voxels it admits);
-// it grows like the table, from a host-side bound of its bricks, with a rehash on the device.  ctr->bricks counts
-// the claimed bricks, so the host can tighten that bound from the counters each insertion mirrors.
-struct DenseLiveIndex {                // device view, by value in the kernel arguments
-  unsigned long long* key;             // brick key per slot, DENSE_EMPTY when free
-  unsigned long long* mask;            // DENSE_BRICK_WORDS words per slot
-  unsigned long long slots_mask;       // slots - 1 (a power of two, load factor <= 0.5)
-};
+// Live occupancy index: a DenseBrickIndex over the live table without base or idx (keys and masks only, so a rehash of
+// the voxel table leaves it valid).  Built from the table when carve mode is switched on, then kept current by the
+// insertion (dense_live_insert_kernel sets the bits of the voxels it admits); it grows like the table, from a host-side
+// bound of its bricks, with a rehash on the device.  ctr->bricks counts the claimed bricks, so the host can tighten
+// that bound from the counters each insertion mirrors.
 
 // set voxel `key`'s bit: find or claim its brick (a claim counts a brick)
-__device__ __forceinline__ void dense_live_set(const DenseLiveIndex& ix, unsigned long long key,
+__device__ __forceinline__ void dense_live_set(const DenseBrickIndex& ix, unsigned long long key,
                                                DenseCounters* __restrict__ ctr) {
-  const unsigned long long c = dense_brick_composite(key), brick = c >> 9;
-  const unsigned bit = (unsigned)(c & 511);
-  unsigned long long h = dense_hash(brick) & ix.slots_mask;
-  for (;;) {
-    const unsigned long long prev = atomicCAS(&ix.key[h], DENSE_EMPTY, brick);
-    if (prev == DENSE_EMPTY) atomicAdd(&ctr->bricks, 1ull);
-    if (prev == DENSE_EMPTY || prev == brick) break;
-    h = (h + 1) & ix.slots_mask;
-  }
-  atomicOr(&ix.mask[h * DENSE_BRICK_WORDS + (bit >> 6)], 1ull << (bit & 63));
+  const unsigned long long c = dense_brick_composite(key);
+  bool claimed = false;
+  const long long h = ix.find_or_claim(c >> 9, &claimed);
+  if (claimed) atomicAdd(&ctr->bricks, 1ull);
+  ix.set(h, (unsigned)(c & 511));
 }
 
 // build: one thread per table slot (carve mode switched on with voxels stored; never on the per-sweep path)
-__global__ void dense_live_build_kernel(const DenseSlot* __restrict__ t, unsigned long long size, DenseLiveIndex ix,
+__global__ void dense_live_build_kernel(const DenseSlot* __restrict__ t, unsigned long long size, DenseBrickIndex ix,
                                         DenseCounters* __restrict__ ctr) {
   const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
   if (i >= size) return;
@@ -859,24 +899,21 @@ __global__ void dense_live_build_kernel(const DenseSlot* __restrict__ t, unsigne
   if (k != DENSE_EMPTY) dense_live_set(ix, k, ctr);
 }
 
-// growth: every brick of the old index moves to the new one with its mask (each brick once: a plain claim)
-__global__ void dense_live_rehash_kernel(const unsigned long long* __restrict__ old_key,
-                                         const unsigned long long* __restrict__ old_mask, unsigned long long old_slots,
-                                         DenseLiveIndex ix) {
+// growth: every brick of the old index moves to the new one with its mask (each brick once)
+__global__ void dense_live_rehash_kernel(DenseBrickIndex old, DenseBrickIndex ix) {
   const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
-  if (i >= old_slots) return;
-  const unsigned long long b = old_key[i];
+  if (i > old.slots_mask) return;
+  const unsigned long long b = old.key[i];
   if (b == DENSE_EMPTY) return;
-  unsigned long long h = dense_hash(b) & ix.slots_mask;
-  while (atomicCAS(&ix.key[h], DENSE_EMPTY, b) != DENSE_EMPTY) h = (h + 1) & ix.slots_mask;
+  const long long h = ix.find_or_claim(b);
 #pragma unroll
-  for (int w = 0; w < DENSE_BRICK_WORDS; w++) ix.mask[h * DENSE_BRICK_WORDS + w] = old_mask[i * DENSE_BRICK_WORDS + w];
+  for (int w = 0; w < DENSE_BRICK_WORDS; w++) ix.mask[h * DENSE_BRICK_WORDS + w] = old.mask[i * DENSE_BRICK_WORDS + w];
 }
 
 // in the insertion, between dense_insert_kernel and dense_finish_kernel: the voxels that kernel admitted (new runs
 // ranked below the room, the same test on the same ctr->voxels) get their bits
 __global__ void dense_live_insert_kernel(DenseRuns runs, const int* __restrict__ n_runs, const unsigned* __restrict__ rank,
-                                         const unsigned* __restrict__ block_off, DenseLiveIndex ix,
+                                         const unsigned* __restrict__ block_off, DenseBrickIndex ix,
                                          DenseCounters* __restrict__ ctr, unsigned long long max_voxels) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= *n_runs || runs.slot[r] != -1) return;
@@ -906,12 +943,11 @@ __global__ void dense_carve_mark_kernel(const float4* __restrict__ p, int n, flo
 
 // One thread per ray (tests/carve_reference.py restates it), fp64 without FMA: e = p - o, r = sqrt((ex*ex + ey*ey) +
 // ez*ez), d = e / r (a non-finite p or r == 0 casts nothing); T = min(r - margin, max_range); DenseWalk from o along d
-// until the first voxel with t_exit > T; every voxel before it that the index holds is carved.  One brick probe per
-// brick entered, one mask word per voxel inside a non-empty brick, a table probe only for an occupied voxel.  The
-// first ray to carve a slot that is not in K moves its stamp to c_code and adds the pass's one miss, so the count
-// depends neither on the thread order nor on how many rays cross the voxel.
+// until the first voxel with t_exit > T; every voxel before it that the index holds is carved, with a table probe only
+// for an occupied voxel.  The first ray to carve a slot that is not in K moves its stamp to c_code and adds the pass's
+// one miss, so the count depends neither on the thread order nor on how many rays cross the voxel.
 __global__ void __launch_bounds__(128)
-dense_carve_kernel(const float4* __restrict__ p, int n, DenseCarveArgs a, DenseRayIndex ix, DenseSlot* t,
+dense_carve_kernel(const float4* __restrict__ p, int n, DenseCarveArgs a, DenseBrickIndex ix, DenseSlot* t,
                    unsigned long long tmask, unsigned* stamp) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -922,32 +958,25 @@ dense_carve_kernel(const float4* __restrict__ p, int n, DenseCarveArgs a, DenseR
   if (!(r > 0.0)) return;
   const double rm = r - a.margin;
   const double T = rm < a.max_range ? rm : a.max_range;
-  DenseWalk w(a.ox, a.oy, a.oz, ex / r, ey / r, ez / r, a.leaf);
-  long long slot = dense_brick_find(ix, w.vx, w.vy, w.vz);
+  DenseWalk w(ix, a.ox, a.oy, a.oz, ex / r, ey / r, ez / r, a.leaf);
   for (int s = 0; s < DENSE_RAY_MAX_STEPS; s++) {
     const int ax = w.axis();
     if (w.t_next(ax) > T) break;
-    if (slot >= 0) {
-      const unsigned bit = dense_local_bit(w.vx, w.vy, w.vz);
-      if ((__ldg(&ix.mask[slot * DENSE_BRICK_WORDS + (bit >> 6)]) >> (bit & 63)) & 1ull) {
-        constexpr int H = 1 << 20;
-        const unsigned long long key = ((unsigned long long)(w.vz + H) << 42) |
-                                       ((unsigned long long)(w.vy + H) << 21) | (unsigned long long)(w.vx + H);
-        const long long ts = dense_find(t, tmask, key);
-        if (ts >= 0) {
-          unsigned old = stamp[ts];
-          while (old != a.k_code && old != a.c_code) {
-            const unsigned prev = atomicCAS(&stamp[ts], old, a.c_code);
-            if (prev == old) {
-              t[ts].evidence = dense_add_miss(t[ts].evidence);
-              break;
-            }
-            old = prev;
+    if (w.slot >= 0 && ix.test(w.slot, w.bit())) {
+      const long long ts = dense_find(t, tmask, dense_key(w.vx, w.vy, w.vz));
+      if (ts >= 0) {
+        unsigned old = stamp[ts];
+        while (old != a.k_code && old != a.c_code) {
+          const unsigned prev = atomicCAS(&stamp[ts], old, a.c_code);
+          if (prev == old) {
+            t[ts].evidence = dense_add_miss(t[ts].evidence);
+            break;
           }
+          old = prev;
         }
       }
     }
-    if (w.step(ax)) slot = dense_brick_find(ix, w.vx, w.vy, w.vz);
+    w.step(ix, ax);
   }
 }
 
@@ -977,9 +1006,8 @@ struct DenseMap {
   int vis_rows = 0, vis_cols = 0;
   DevBuf<unsigned> image;         // range image of the sweep being observed (float bits, DENSE_NO_RETURN when empty)
   double carve_margin = 0.0, carve_max = 0.0;  // carve mode (carve_max == 0: off)
-  unsigned long long* live_key = nullptr;      // carve mode's occupancy index (stream-ordered allocations on `stream`)
-  unsigned long long* live_mask = nullptr;
-  unsigned long long live_slots = 0;           // 0: no index (carve mode off, or dropped by a clear)
+  DenseBrickIndex live;                        // carve mode's occupancy index (stream-ordered allocations on `stream`;
+                                               // no slots: carve mode off, or dropped by a clear)
   unsigned long long live_bound = 0;           // upper bound of its bricks, known without a readback
   unsigned* stamp = nullptr;                   // carve mode's per-slot stamps (table_size words once allocated)
   unsigned long long stamp_size = 0;
@@ -995,8 +1023,8 @@ struct DenseMap {
     if (stream) {
       cudaStreamSynchronize(stream);
       if (table) cudaFreeAsync(table, stream);
-      if (live_key) cudaFreeAsync(live_key, stream);
-      if (live_mask) cudaFreeAsync(live_mask, stream);
+      if (live.key) cudaFreeAsync(live.key, stream);
+      if (live.mask) cudaFreeAsync(live.mask, stream);
       if (stamp) cudaFreeAsync(stamp, stream);
       cudaStreamSynchronize(stream);
       cudaStreamDestroy(stream);
@@ -1004,8 +1032,8 @@ struct DenseMap {
     stream = nullptr;
     table = nullptr;
     table_size = 0;
-    live_key = live_mask = nullptr;
-    live_slots = live_bound = 0;
+    live = DenseBrickIndex{};
+    live_bound = 0;
     stamp = nullptr;
     stamp_size = 0;
     sort.keys_a.release(); sort.keys_b.release(); sort.vals_a.release(); sort.vals_b.release(); sort.hist.release();
@@ -1036,8 +1064,10 @@ struct DenseTarget {
   DevBuf<int> match, flag;
   DevBuf<float4> coeff;
   DevBuf<int8_t> sel;
-  // ray index of loam_b200_dense_raycast: built on the first cast after a build or load (ray_slots > 0 once built)
-  unsigned long long ray_slots = 0;
+  // ray index of loam_b200_dense_raycast: built on the first cast after a build or load (slots once built).  Its
+  // pointers alias the ray_* buffers below, so those are reserved only by dense_ray_index_build, which runs only while
+  // `ray` is empty (a build, load or release empties it first).
+  DenseBrickIndex ray;
   DevBuf<unsigned long long> ray_key, ray_mask;
   DevBuf<unsigned> ray_base;
   DevBuf<int> ray_idx;
@@ -1049,7 +1079,7 @@ struct DenseTarget {
     result.release(); ticket.release(); match.release(); flag.release(); coeff.release(); sel.release();
     ray_key.release(); ray_mask.release(); ray_base.release(); ray_idx.release(); ray_range.release();
     ray_hit.release();
-    ray_slots = 0;
+    ray = DenseBrickIndex{};
     n = 0;
     ready = false;
   }

@@ -620,6 +620,102 @@ int loam_b200_dense_raycast(loam_b200_ctx* ctx, const float* rays, int n, int on
 int loam_b200_debug_dense_ray_index_bytes(loam_b200_ctx* ctx, long long* out);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Place recognition and global relocalisation in the whole-run voxel map (csrc/densemap.cuh, DESIGN.md "Place
+ * recognition and global relocalisation"): relocalise a cloud with no prior pose -- a robot waking up in a saved map,
+ * a tracking loss after a long gap, a second session that starts elsewhere.  A polar height descriptor of the cloud
+ * is compared with descriptors rendered from the target at candidate places, over every heading; the best places,
+ * each with a heading, become a small dense_relocalize grid.  Not on the per-sweep path.
+ *   Descriptor (rings x sectors cells, ring-major, float), LOAM frame: y is up, the ground plane x-z, heading rot_y.
+ *     Per point (float[4] in the sensor frame, w ignored), fp64 without FMA, each operation rounded on its own:
+ *       a non-finite point is skipped; r = sqrt(x*x + z*z); skipped when r == 0 or r >= max_radius;
+ *       ring = floor(r / w) with w = (double)max_radius / rings on the host, clamped to rings - 1;
+ *       sector: the wedge [k D, (k + 1) D), D = (2 pi) / sectors in double, that holds the azimuth atan2(x, z), found
+ *         without a transcendental function on the device: the number of boundaries k in [1, sectors) that the point
+ *         is at or past, where past(k) = h_p > h_k, or h_p == h_k and x * cos(k D) - z * sin(k D) >= 0; h_k = 1 when
+ *         2k >= sectors (else 0), h_p = 0 when x > 0 or (x == 0 and z > 0) (else 1); cos / sin are std::cos /
+ *         std::sin in double of (double)k * D on the host, except (-1, 0) exactly for the boundary at pi (2k ==
+ *         sectors).  past() then holds on a prefix of the boundaries, so the device bisects;
+ *       value v = (float)(y + height_offset); a point with v not in (0, FLT_MAX] is skipped.
+ *     A cell holds the largest value of its points, 0 when it has none.  Bit-reproducible in any thread order.
+ *     Headings: to_map rotates a sensor-frame azimuth phi to phi + rot_y, so query column j matching database column
+ *     (j + s) mod sectors means heading s D, reported wrapped to (-pi, pi]: yaw = (float)((double)a * D) with a = s
+ *     when 2s <= sectors, else s - sectors.
+ *   place_descriptor: the descriptor of n points (host, or device when on_device != 0) -> out[rings * sectors].
+ *   dense_place_build: the place database of the current target: k candidate positions (float[3], map frame) and
+ *     n_rays sensor-frame rays (float[4]: lidar_rays with the query sensor's elevations and an azimuth count that is
+ *     a multiple of sectors).  Candidate c's descriptor is, by definition, place_descriptor of the points
+ *     (float)((double)range_i * u_i) per axis over the rays i that hit, where (range, u) are loam_b200_dense_raycast's
+ *     from the pose rot = 0, pos = positions[c] with params.min_range / max_range (u = p / |p| of that call).  Rendering
+ *     through the cast keeps occlusion.  The ray index is built first when absent.  The database belongs to the
+ *     target: the next target build or load drops it, later inserts do not change it; it is a function of (target,
+ *     positions, rays, params), so a loaded target and the saved positions rebuild it exactly.  A build replaces the
+ *     previous database.  LOAM_B200_ERR_ARG: 1 <= rings <= 64, 1 <= sectors <= 720, rings * sectors <= 4096, max_radius
+ *     finite > 0, height_offset finite, the cast's range rules (0 <= min_range < max_range, finite, max_range / leaf
+ *     <= 65536), 1 <= k <= 1 << 20, every position finite with its voxel in the key range, n_rays >= 0, no NULL
+ *     pointer.  LOAM_B200_ERR_CAPACITY: k * rings * sectors * 4 bytes above LOAM_B200_PLACE_MAX_BYTES.
+ *   dense_place_query: the descriptor of the cloud (as place_descriptor, with the database's params), then every
+ *     candidate at every shift s in [0, sectors): per column j ascending, query column j against candidate column
+ *     (j + s) mod sectors; qq, dd and dot are fp64 sums in ascending ring; a column with qq == 0 or dd == 0 is
+ *     skipped, otherwise sim = dot / (sqrt(qq) * sqrt(dd)) is added; dist = 1 - sum / counted (+inf when none is
+ *     counted).  Per candidate the best shift: smallest dist, ties to the smaller s.  out: the top_m (1..1024)
+ *     candidates by dist ascending, then index ascending, never one at +inf; *n_out = entries written.  No database:
+ *     LOAM_B200_ERR_STATE.
+ *   place_grid: host only.  For each match m in order, loam_b200_reloc_grid of the prior (rot = (0, yaw_m, 0), pos =
+ *     pos_m) with the given steps, concatenated; *n_out = the total (LOAM_B200_ERR_CAPACITY above cap, LOAM_B200_ERR_ARG
+ *     above 1 << 20 or for the grid's argument errors).
+ *   dense_relocalize_global: dense_place_query(top_m), then loam_b200_dense_relocalize on the place_grid of its
+ *     matches -- bit for bit that call on that list; a host cloud is uploaded once.  A candidate's hypothesis indexes
+ *     the list, so its match is hypothesis / ((2 yaw_steps + 1) (2 xz_steps + 1)^2); query + place_grid regenerate the
+ *     list.  No match: no candidate.  Errors are those of the three calls.
+ *   Launches count under LOAM_B200_K_DENSE.  With none of these called nothing is launched, allocated or recorded.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int rings;           /* N_r, 1..64 */
+  int sectors;         /* N_s, 1..720, rings * sectors <= 4096 */
+  float max_radius;    /* metres, > 0 */
+  float height_offset; /* metres added to y before the value (the sensor's height above the ground, or more) */
+  float min_range;     /* the database's cast: loam_b200_dense_raycast's min_range ... */
+  float max_range;     /* ... and max_range */
+} loam_b200_place_params;
+
+typedef struct {
+  int candidate; /* index into the positions of dense_place_build */
+  int shift;     /* the best shift s */
+  float yaw;     /* its heading s D wrapped to (-pi, pi] */
+  float pos[3];  /* the candidate's position */
+  double dist;   /* its distance */
+} loam_b200_place_match;
+
+/* Recommended parameters, chosen from the recall measured on route maps (DESIGN.md "Place recognition and global
+ * relocalisation"): 20 rings, 60 sectors (6 deg), 80 m, height offset 2 m, the database cast from 0 to 100 m; places
+ * every 4 m along the route; the global relocalisation refines the 5 best places over +-3 steps of 2 deg and an x-z
+ * grid of 0.4 m steps five to each side (+-2 m): 5 x 7 x 121 = 4235 poses. */
+#define LOAM_B200_PLACE_PARAMS_DEFAULT {20, 60, 80.0f, 2.0f, 0.0f, 100.0f}
+#define LOAM_B200_PLACE_SPACING 4.0f
+#define LOAM_B200_PLACE_TOP_M 5
+#define LOAM_B200_PLACE_YAW_STEP_DEG 2.0f
+#define LOAM_B200_PLACE_YAW_STEPS 3
+#define LOAM_B200_PLACE_XZ_STEP 0.4f
+#define LOAM_B200_PLACE_XZ_STEPS 5
+#define LOAM_B200_PLACE_MAX_BYTES (1ll << 30)
+
+int loam_b200_place_descriptor(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device,
+                               const loam_b200_place_params* prm, float* out);
+int loam_b200_dense_place_build(loam_b200_ctx* ctx, const float* positions, int k, const float* rays, int n_rays,
+                                const loam_b200_place_params* prm);
+int loam_b200_dense_place_query(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device, int top_m,
+                                loam_b200_place_match* out, int* n_out);
+int loam_b200_place_grid(const loam_b200_place_match* matches, int n_matches, float yaw_step_deg, int yaw_steps,
+                         float xz_step, int xz_steps, loam_b200_pose* out, int cap, int* n_out);
+int loam_b200_dense_relocalize_global(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device, int top_m,
+                                      float yaw_step_deg, int yaw_steps, float xz_step, int xz_steps,
+                                      const loam_b200_reloc_params* prm, loam_b200_reloc_candidate* out, int cap,
+                                      int* n_out);
+/* Test query: the database's descriptors, k * rings * sectors floats in candidate order -> out; *n_out = that count
+ * (0 without a database), LOAM_B200_ERR_CAPACITY when it exceeds cap. */
+int loam_b200_debug_dense_place_descriptors(loam_b200_ctx* ctx, float* out, long long cap, long long* n_out);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice
  * of the corner and surface queries; with a communicator the 32-float partial normal equations are all-reduced
  * (NCCL, sum, fp32) on the context's stream directly behind the kernel, so every rank returns the same totals and

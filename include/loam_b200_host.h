@@ -145,6 +145,17 @@ int loam_b200_map_dense_relocalize(void* h, const float* xyzi, int n, const floa
  * NULL). */
 int loam_b200_map_dense_raycast(void* h, const float* rays, int n, const float* pose6, float min_range,
                                 float max_range, float* range, int* index);
+/* place recognition and global relocalisation in that target (BasicLaserMapping::buildDensePlaces /
+ * queryDensePlaces / relocalizeGlobalInDenseTarget, include/loam_b200.h "Place recognition and global
+ * relocalisation"), same in-flight rule: k positions of float[3], n_rays rays and n points of float[4]. */
+int loam_b200_map_dense_place_build(void* h, const float* positions, int k, const float* rays, int n_rays,
+                                    const loam_b200_place_params* prm);
+int loam_b200_map_dense_place_query(void* h, const float* xyzi, int n, int top_m, loam_b200_place_match* out,
+                                    int* n_out);
+int loam_b200_map_dense_relocalize_global(void* h, const float* xyzi, int n, int top_m, float yaw_step_deg,
+                                          int yaw_steps, float xz_step, int xz_steps,
+                                          const loam_b200_reloc_params* prm, loam_b200_reloc_candidate* out, int cap,
+                                          int* n_out);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank
  * then enables sharding on its mapping object (nccl_id128 = NULL: slice the queries only, no collective) */
 int loam_b200_host_nccl_unique_id(unsigned char* out128);

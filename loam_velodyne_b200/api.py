@@ -85,6 +85,26 @@ class RelocCandidate(C.Structure):
 RELOC_YAW_STEP_DEG, RELOC_XZ_STEP, RELOC_XZ_STEPS = 2.0, 0.4, 4
 
 
+class PlaceParams(C.Structure):
+    """loam_b200_place_params; default(): the recommended parameters (LOAM_B200_PLACE_PARAMS_DEFAULT)."""
+    _fields_ = [("rings", C.c_int), ("sectors", C.c_int), ("max_radius", C.c_float), ("height_offset", C.c_float),
+                ("min_range", C.c_float), ("max_range", C.c_float)]
+
+    @staticmethod
+    def default():
+        return PlaceParams(20, 60, np.float32(80.0), np.float32(2.0), np.float32(0.0), np.float32(100.0))
+
+
+class PlaceMatch(C.Structure):
+    _fields_ = [("candidate", C.c_int), ("shift", C.c_int), ("yaw", C.c_float), ("pos", C.c_float * 3),
+                ("dist", C.c_double)]
+
+
+# recommended place spacing and global relocalisation grid (include/loam_b200.h LOAM_B200_PLACE_*)
+PLACE_SPACING, PLACE_TOP_M = 4.0, 5
+PLACE_YAW_STEP_DEG, PLACE_YAW_STEPS, PLACE_XZ_STEP, PLACE_XZ_STEPS = 2.0, 3, 0.4, 5
+
+
 class NormalEq(C.Structure):
     _fields_ = [("AtA", C.c_float * 36), ("AtB", C.c_float * 6), ("n_selected", C.c_int),
                 ("n_corner_selected", C.c_int)]
@@ -210,6 +230,15 @@ def lib():
                                                  C.POINTER(RelocParams), C.POINTER(RelocCandidate), C.c_int, _I]),
         "loam_b200_dense_raycast": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_float, C.c_float, _F, _I]),
         "loam_b200_debug_dense_ray_index_bytes": (C.c_int, [vp, _LL]),
+        "loam_b200_place_descriptor": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(PlaceParams), _F]),
+        "loam_b200_dense_place_build": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.POINTER(PlaceParams)]),
+        "loam_b200_dense_place_query": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_int, C.POINTER(PlaceMatch), _I]),
+        "loam_b200_place_grid": (C.c_int, [C.POINTER(PlaceMatch), C.c_int, C.c_float, C.c_int, C.c_float, C.c_int,
+                                           C.POINTER(Pose), C.c_int, _I]),
+        "loam_b200_dense_relocalize_global": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
+                                                        C.c_float, C.c_int, C.POINTER(RelocParams),
+                                                        C.POINTER(RelocCandidate), C.c_int, _I]),
+        "loam_b200_debug_dense_place_descriptors": (C.c_int, [vp, _F, C.c_longlong, _LL]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -271,6 +300,11 @@ def lib():
         "loam_b200_map_dense_relocalize": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.POINTER(RelocParams),
                                                      C.POINTER(RelocCandidate), C.c_int, _I]),
         "loam_b200_map_dense_raycast": (C.c_int, [vp, _F, C.c_int, _F, C.c_float, C.c_float, _F, _I]),
+        "loam_b200_map_dense_place_build": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.POINTER(PlaceParams)]),
+        "loam_b200_map_dense_place_query": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(PlaceMatch), _I]),
+        "loam_b200_map_dense_relocalize_global": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_float, C.c_int, C.c_float,
+                                                            C.c_int, C.POINTER(RelocParams),
+                                                            C.POINTER(RelocCandidate), C.c_int, _I]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_map_kernel_profile": (C.c_int, [vp, C.c_int, _D]),
@@ -799,6 +833,61 @@ class Ctx:
         self._ck(self.L.loam_b200_debug_dense_ray_index_bytes(self.h, C.byref(out)), "dense_ray_index_bytes")
         return out.value
 
+    # ---- place recognition (include/loam_b200.h "Place recognition and global relocalisation")
+    def place_descriptor(self, pts, params=None, on_device=False, n=None):
+        """Polar height descriptor of sensor-frame pts (N x 4, w ignored) -> float32 (rings, sectors).  With
+        on_device=True, pts is the address of n float[4] in device memory."""
+        prm = params if params is not None else PlaceParams.default()
+        ptr, k = _pts_or_device(pts, on_device, n)
+        out = np.zeros((prm.rings, prm.sectors), np.float32)
+        self._ck(self.L.loam_b200_place_descriptor(self.h, ptr, k, 1 if on_device else 0, C.byref(prm), _fp(out)),
+                 "place_descriptor")
+        return out
+
+    def dense_place_build(self, positions, rays, params=None):
+        """The place database of the target: one descriptor per position (K x 3, map frame), rendered through
+        dense_raycast of rays (N x 4, e.g. lidar_rays) from that position with rot = 0."""
+        prm = params if params is not None else PlaceParams.default()
+        p = np.ascontiguousarray(positions, np.float32).reshape(-1, 3)
+        r = _pts(rays)
+        self._ck(self.L.loam_b200_dense_place_build(self.h, _fp(p), p.shape[0], _fp(r), r.shape[0], C.byref(prm)),
+                 "dense_place_build")
+
+    def dense_place_query(self, pts, top_m=PLACE_TOP_M, on_device=False, n=None):
+        """The top_m places for sensor-frame pts -> list of dicts: candidate, shift, yaw, pos (float32[3]), dist."""
+        ptr, k = _pts_or_device(pts, on_device, n)
+        out = (PlaceMatch * max(int(top_m), 1))()
+        got = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_place_query(self.h, ptr, k, 1 if on_device else 0, int(top_m), out,
+                                                    C.byref(got)), "dense_place_query")
+        return [_place_match(m) for m in out[:got.value]]
+
+    def dense_relocalize_global(self, pts, top_m=PLACE_TOP_M, yaw_step_deg=PLACE_YAW_STEP_DEG,
+                                yaw_steps=PLACE_YAW_STEPS, xz_step=PLACE_XZ_STEP, xz_steps=PLACE_XZ_STEPS,
+                                params=None, cap=16):
+        """Relocalise pts with no prior: dense_place_query(top_m), then dense_relocalize over place_grid of its
+        matches -> what dense_relocalize returns; a candidate's hypothesis indexes that grid."""
+        a = _pts(pts)
+        prm = params if params is not None else RelocParams.default()
+        out = (RelocCandidate * max(int(cap), 1))()
+        got = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_relocalize_global(self.h, _fp(a), a.shape[0], 0, int(top_m),
+                                                          np.float32(yaw_step_deg), int(yaw_steps),
+                                                          np.float32(xz_step), int(xz_steps), C.byref(prm), out,
+                                                          int(cap), C.byref(got)), "dense_relocalize_global")
+        return [_candidate(r) for r in out[:got.value]]
+
+    def dense_place_descriptors(self):
+        """Test query: the database's descriptors -> float32 (K, rings, sectors) (K = 0 without a database)."""
+        n = C.c_longlong(0)
+        rc = self.L.loam_b200_debug_dense_place_descriptors(self.h, None, 0, C.byref(n))
+        if rc not in (0, -5):
+            self._ck(rc, "dense_place_descriptors")
+        out = np.zeros(max(n.value, 1), np.float32)
+        self._ck(self.L.loam_b200_debug_dense_place_descriptors(self.h, _fp(out), n.value, C.byref(n)),
+                 "dense_place_descriptors")
+        return out[:n.value].copy()
+
     def profile(self, on=True):
         self.L.loam_b200_profile_enable(self.h, 1 if on else 0)
         self.L.loam_b200_profile_reset(self.h)
@@ -876,6 +965,19 @@ def _candidate(r):
             "fine": _align_out(list(r.fine.rot) + list(r.fine.pos), r.fine.iterations, r.fine.n_selected, r.fine.rms,
                                r.fine.degenerate, r.fine.converged),
             "selected": int(r.selected), "rms": np.float32(r.rms)}
+
+
+def _pts_or_device(pts, on_device, n):
+    """(float pointer, count) of a host N x 4 array, or of a device address of n float[4]."""
+    if on_device:
+        return C.cast(C.c_void_p(int(pts)), _F), int(n)
+    a = _pts(pts)
+    return _fp(a), a.shape[0]
+
+
+def _place_match(m):
+    return {"candidate": int(m.candidate), "shift": int(m.shift), "yaw": np.float32(m.yaw),
+            "pos": np.array(m.pos, np.float32), "dist": float(m.dist)}
 
 
 def _ne(ne: NormalEq):
@@ -1141,6 +1243,38 @@ class LaserMapping(_Handle):
                                                     np.float32(max_range), _fp(rng), _ip(idx)), "raycastDenseTarget")
         return rng[:k].copy(), idx[:k].copy()
 
+    def build_dense_places(self, positions, rays, params=None):
+        """BasicLaserMapping::buildDensePlaces; as Ctx.dense_place_build."""
+        prm = params if params is not None else PlaceParams.default()
+        p = np.ascontiguousarray(positions, np.float32).reshape(-1, 3)
+        r = _pts(rays)
+        self._ck(self.L.loam_b200_map_dense_place_build(self.h, _fp(p), p.shape[0], _fp(r), r.shape[0],
+                                                        C.byref(prm)), "buildDensePlaces")
+
+    def query_dense_places(self, pts, top_m=PLACE_TOP_M):
+        """BasicLaserMapping::queryDensePlaces; returns what Ctx.dense_place_query returns."""
+        a = _pts(pts)
+        out = (PlaceMatch * max(int(top_m), 1))()
+        got = C.c_int(0)
+        self._ck(self.L.loam_b200_map_dense_place_query(self.h, _fp(a), a.shape[0], int(top_m), out, C.byref(got)),
+                 "queryDensePlaces")
+        return [_place_match(m) for m in out[:got.value]]
+
+    def relocalize_global_in_dense_target(self, pts, top_m=PLACE_TOP_M, yaw_step_deg=PLACE_YAW_STEP_DEG,
+                                          yaw_steps=PLACE_YAW_STEPS, xz_step=PLACE_XZ_STEP, xz_steps=PLACE_XZ_STEPS,
+                                          params=None, cap=16):
+        """BasicLaserMapping::relocalizeGlobalInDenseTarget; returns what Ctx.dense_relocalize_global returns."""
+        a = _pts(pts)
+        prm = params if params is not None else RelocParams.default()
+        out = (RelocCandidate * max(int(cap), 1))()
+        got = C.c_int(0)
+        self._ck(self.L.loam_b200_map_dense_relocalize_global(self.h, _fp(a), a.shape[0], int(top_m),
+                                                              np.float32(yaw_step_deg), int(yaw_steps),
+                                                              np.float32(xz_step), int(xz_steps), C.byref(prm), out,
+                                                              int(cap), C.byref(got)),
+                 "relocalizeGlobalInDenseTarget")
+        return [_candidate(r) for r in out[:got.value]]
+
     def enable_dense_visibility(self, h_res_deg, v_res_deg, margin):
         """Count, per voxel of the whole-run map, the mapped sweeps that see through it (h_res_deg = 0: off); filter
         with dense_map(max_miss_ratio=...)."""
@@ -1368,6 +1502,38 @@ def lidar_rays(elevations_deg, n_az):
     d = np.stack([-np.sin(theta) * np.cos(e), np.broadcast_to(np.sin(e), (e.shape[0], int(n_az))),
                   np.cos(theta) * np.cos(e), np.zeros((e.shape[0], int(n_az)))], axis=-1)
     return np.ascontiguousarray(d.reshape(-1, 4), np.float32)
+
+
+def place_grid(matches, yaw_step_deg=PLACE_YAW_STEP_DEG, yaw_steps=PLACE_YAW_STEPS, xz_step=PLACE_XZ_STEP,
+               xz_steps=PLACE_XZ_STEPS):
+    """loam_b200_place_grid (host only): the hypothesis list of dense_relocalize_global for the matches of
+    dense_place_query (dicts) -> K x 6 float32 twists, reloc_grid around each match in order."""
+    L = lib()
+    ms = (PlaceMatch * max(len(matches), 1))()
+    for i, m in enumerate(matches):
+        ms[i].candidate, ms[i].shift, ms[i].yaw, ms[i].dist = m["candidate"], m["shift"], m["yaw"], m["dist"]
+        for e in range(3):
+            ms[i].pos[e] = m["pos"][e]
+    n = C.c_int(0)
+    args = (ms, len(matches), np.float32(yaw_step_deg), int(yaw_steps), np.float32(xz_step), int(xz_steps))
+    rc = L.loam_b200_place_grid(*args, None, 0, C.byref(n))
+    if rc not in (0, -5):  # LOAM_B200_ERR_CAPACITY: the count is in n
+        raise LoamB200Error(f"place_grid: {L.loam_b200_strerror(rc).decode()}")
+    out = (Pose * max(n.value, 1))()
+    if L.loam_b200_place_grid(*args, out, n.value, C.byref(n)) != 0:
+        raise LoamB200Error("place_grid failed")
+    return np.array([list(p.rot) + list(p.pos) for p in out[:n.value]], np.float32).reshape(-1, 6)
+
+
+def thin_trajectory(positions, spacing=PLACE_SPACING):
+    """Places for dense_place_build from a trajectory (K x 3, in driving order): the first position, then every
+    position at least `spacing` metres (straight line) from the last one kept -> M x 3 float32."""
+    p = np.ascontiguousarray(positions, np.float32).reshape(-1, 3)
+    keep = []
+    for i in range(p.shape[0]):
+        if not keep or np.linalg.norm(p[i].astype(np.float64) - p[keep[-1]].astype(np.float64)) >= spacing:
+            keep.append(i)
+    return p[keep].copy()
 
 
 def nccl_unique_id() -> bytes:

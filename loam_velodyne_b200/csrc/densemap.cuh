@@ -24,6 +24,7 @@
 #pragma once
 
 #include <cmath>
+#include <vector>
 
 #include "linalg.cuh"
 #include "mapping_lm.cuh"
@@ -813,6 +814,52 @@ struct DenseWalk {
 //   t_exit > min_range is the hit, at t = clamp(num / den, lo, hi) on its surfel (den != 0) or lo (no normal, or
 //   den == 0), lo = max(t_enter, min_range), hi = t_exit; t > max_range is no hit.  Then one step along the axis of the
 //   smallest t_next (ties x, y, z); t_enter = its old t_next; only its t_next is recomputed, from the new index.
+// dense_ray_hit is the walk and hit from origin (ox, oy, oz) along the map-frame unit d: the hit's target index and *t,
+// or -1.  It is the one copy of the rule; dense_raycast_kernel and dense_place_build_kernel both run it.
+__device__ __forceinline__ int dense_ray_hit(const DenseBrickIndex& ix, const float4* __restrict__ cent,
+                                             const float4* __restrict__ nrm, double ox, double oy, double oz, double dx,
+                                             double dy, double dz, double leaf, double min_range, double max_range,
+                                             double* t_out) {
+  DenseWalk w(ix, ox, oy, oz, dx, dy, dz, leaf);
+  double t_enter = 0.0, lo = 0.0, hi = 0.0;
+  int j_hit = -1;
+  for (int s = 0; s < DENSE_RAY_MAX_STEPS; s++) {
+    if (t_enter > max_range) break;
+    const int ax = w.axis();
+    const double t_exit = w.t_next(ax);
+    if (w.slot >= 0 && t_exit > min_range) {
+      const unsigned bit = w.bit();
+      if (ix.test(w.slot, bit)) {  // its target index: the brick's voxels below it, after the brick's base
+        const unsigned long long* m = ix.mask + w.slot * DENSE_BRICK_WORDS;
+        int below = __popcll(ix.word(w.slot, bit) & ((1ull << (bit & 63)) - 1ull));
+        for (unsigned k = 0; k < (bit >> 6); k++) below += __popcll(__ldg(&m[k]));
+        j_hit = __ldg(&ix.idx[__ldg(&ix.base[w.slot]) + below]);
+        lo = t_enter > min_range ? t_enter : min_range;
+        hi = t_exit;
+        break;
+      }
+    }
+    t_enter = t_exit;
+    w.step(ix, ax);
+  }
+  if (j_hit < 0) return -1;
+  double t = lo;  // the surfel range, outside the walk (its division stays out of the loop)
+  const float4 nv = nrm[j_hit];
+  if (!isnan(nv.x)) {
+    const double den = ((double)nv.x * dx + (double)nv.y * dy) + (double)nv.z * dz;
+    if (den != 0.0) {
+      const float4 c = cent[j_hit];
+      const double num = ((double)nv.x * ((double)c.x - ox) + (double)nv.y * ((double)c.y - oy)) +
+                         (double)nv.z * ((double)c.z - oz);
+      const double q = num / den;
+      t = q < lo ? lo : (q > hi ? hi : q);
+    }
+  }
+  if (t > max_range) return -1;
+  *t_out = t;
+  return j_hit;
+}
+
 __global__ void
 dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, DenseBrickIndex ix,
                      const float4* __restrict__ cent, const float4* __restrict__ nrm, float* __restrict__ range,
@@ -827,50 +874,192 @@ dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, Den
     const double x1 = a.cz * ux - a.sz * uy, y1 = a.sz * ux + a.cz * uy;
     const double y2 = a.cx * y1 - a.sx * uz, z2 = a.sx * y1 + a.cx * uz;
     const double dx = a.cy * x1 + a.sy * z2, dy = y2, dz = a.cy * z2 - a.sy * x1;
-    DenseWalk w(ix, a.ox, a.oy, a.oz, dx, dy, dz, a.leaf);
-    double t_enter = 0.0, lo = 0.0, hi = 0.0;
-    int j_hit = -1;
-    for (int s = 0; s < DENSE_RAY_MAX_STEPS; s++) {
-      if (t_enter > a.max_range) break;
-      const int ax = w.axis();
-      const double t_exit = w.t_next(ax);
-      if (w.slot >= 0 && t_exit > a.min_range) {
-        const unsigned bit = w.bit();
-        if (ix.test(w.slot, bit)) {  // its target index: the brick's voxels below it, after the brick's base
-          const unsigned long long* m = ix.mask + w.slot * DENSE_BRICK_WORDS;
-          int below = __popcll(ix.word(w.slot, bit) & ((1ull << (bit & 63)) - 1ull));
-          for (unsigned k = 0; k < (bit >> 6); k++) below += __popcll(__ldg(&m[k]));
-          j_hit = __ldg(&ix.idx[__ldg(&ix.base[w.slot]) + below]);
-          lo = t_enter > a.min_range ? t_enter : a.min_range;
-          hi = t_exit;
-          break;
-        }
-      }
-      t_enter = t_exit;
-      w.step(ix, ax);
-    }
-    if (j_hit >= 0) {  // the surfel range, outside the walk (its division stays out of the loop)
-      double t = lo;
-      const float4 nv = nrm[j_hit];
-      if (!isnan(nv.x)) {
-        const double den = ((double)nv.x * dx + (double)nv.y * dy) + (double)nv.z * dz;
-        if (den != 0.0) {
-          const float4 c = cent[j_hit];
-          const double num = ((double)nv.x * ((double)c.x - a.ox) + (double)nv.y * ((double)c.y - a.oy)) +
-                             (double)nv.z * ((double)c.z - a.oz);
-          const double q = num / den;
-          t = q < lo ? lo : (q > hi ? hi : q);
-        }
-      }
-      if (!(t > a.max_range)) {
-        range[i] = (float)t;
-        index[i] = j_hit;
-        return;
-      }
+    double t;
+    const int j_hit = dense_ray_hit(ix, cent, nrm, a.ox, a.oy, a.oz, dx, dy, dz, a.leaf, a.min_range, a.max_range, &t);
+    if (j_hit >= 0) {
+      range[i] = (float)t;
+      index[i] = j_hit;
+      return;
     }
   }
   range[i] = __int_as_float(0x7f800000);  // no hit
   index[i] = -1;
+}
+
+// ---- place descriptors and global relocalisation (include/loam_b200.h "Place recognition")
+// Polar height descriptor, rings x sectors cells (ring-major), each the float bits of the largest value v > 0 of its
+// points (0: none).  Bits of non-negative floats order like the floats, so atomicMax gives the same cell in any order.
+constexpr int DENSE_PLACE_MAX_RINGS = 64;
+constexpr int DENSE_PLACE_MAX_SECTORS = 720;
+constexpr int DENSE_PLACE_MAX_CELLS = 4096;  // the descriptor of one CTA in shared memory
+constexpr int DENSE_PLACE_THREADS = 256;
+
+struct DensePlaceArgs {  // by value in the kernel arguments
+  double ring_w;         // max_radius / rings (host, double)
+  double max_radius, height_offset;
+  int rings, sectors;
+};
+
+// The cell of one sensor-frame point and its value's bits, or -1 (fp64 without FMA; tests/place_reference.py restates
+// it): a non-finite point, r = sqrt(x*x + z*z) == 0 or r >= max_radius, or v = (float)(y + height_offset) not in
+// (0, FLT_MAX] has none.  ring = min(floor(r / ring_w), rings - 1).  Sector: the number of boundaries k in
+// [1, sectors) the point is at or past, past(k) = h_p > h_k, or h_p == h_k and x * tab[k].x - z * tab[k].y >= 0, with
+// h_k = (2k >= sectors), h_p = 0 when x > 0 or (x == 0 and z > 0), else 1; tab[k] = (cos, sin) of k D, the boundary
+// at pi exactly (-1, 0).  past() holds on a prefix of the boundaries (they lie at least 0.5 deg apart, far beyond
+// the rounding of the test, and no point of a half is antipodal to a boundary of its half), so bisection finds the
+// count.
+__device__ __forceinline__ int dense_place_cell(const DensePlaceArgs& pa, const double2* __restrict__ tab, float fx,
+                                                float fy, float fz, unsigned* bits) {
+  if (!(isfinite(fx) && isfinite(fy) && isfinite(fz))) return -1;
+  const double x = (double)fx, y = (double)fy, z = (double)fz;
+  const double r = sqrt(x * x + z * z);
+  if (r == 0.0 || !(r < pa.max_radius)) return -1;
+  const float v = (float)(y + pa.height_offset);
+  if (!(v > 0.f && v <= 3.402823466e38f)) return -1;
+  int ring = (int)floor(r / pa.ring_w);
+  if (ring > pa.rings - 1) ring = pa.rings - 1;
+  const int hp = (x > 0.0 || (x == 0.0 && z > 0.0)) ? 0 : 1;
+  int lo = 1, hi = pa.sectors;  // past(k) for every k < lo, !past(k) for every k >= hi
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    const double2 cs = __ldg(&tab[mid]);
+    const int hk = 2 * mid >= pa.sectors ? 1 : 0;
+    if (hp > hk || (hp == hk && x * cs.x - z * cs.y >= 0.0)) lo = mid + 1;
+    else hi = mid;
+  }
+  *bits = __float_as_uint(v);
+  return ring * pa.sectors + (lo - 1);
+}
+
+// the CTA's descriptor (shared, zeroed by the caller) -> atomicMax into the global one
+__device__ __forceinline__ void dense_place_flush(const unsigned* s_desc, unsigned* __restrict__ desc, int cells) {
+  __syncthreads();
+  for (int k = threadIdx.x; k < cells; k += blockDim.x)
+    if (s_desc[k]) atomicMax(&desc[k], s_desc[k]);
+}
+
+__device__ __forceinline__ void dense_place_zero(unsigned* s_desc, int cells) {
+  for (int k = threadIdx.x; k < cells; k += blockDim.x) s_desc[k] = 0u;
+  __syncthreads();
+}
+
+// query: one thread per point into the CTA's descriptor, then one flush per CTA (desc zeroed before the launch)
+__global__ void __launch_bounds__(DENSE_PLACE_THREADS)
+dense_place_bin_kernel(const float4* __restrict__ p, int n, DensePlaceArgs pa, const double2* __restrict__ tab,
+                       unsigned* __restrict__ desc) {
+  __shared__ unsigned s_desc[DENSE_PLACE_MAX_CELLS];
+  const int cells = pa.rings * pa.sectors;
+  dense_place_zero(s_desc, cells);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) {
+    const float4 q = p[i];
+    unsigned b;
+    const int cell = dense_place_cell(pa, tab, q.x, q.y, q.z, &b);
+    if (cell >= 0) atomicMax(&s_desc[cell], b);
+  }
+  dense_place_flush(s_desc, desc, cells);
+}
+
+// database: blockIdx.y = candidate c0 + y, one thread per ray (dense_raycast_kernel's u and dense_ray_hit from the
+// candidate's float position with rot = 0, so d = u), the hit's point (float)((double)(float)t * u_a) per axis binned
+// by dense_place_cell; desc (zeroed before the launch) holds one descriptor per candidate
+__global__ void __launch_bounds__(DENSE_PLACE_THREADS)
+dense_place_build_kernel(const float4* __restrict__ rays, int n, const float* __restrict__ pos, int c0, DenseRayArgs a,
+                         DenseBrickIndex ix, const float4* __restrict__ cent, const float4* __restrict__ nrm,
+                         DensePlaceArgs pa, const double2* __restrict__ tab, unsigned* __restrict__ desc) {
+  __shared__ unsigned s_desc[DENSE_PLACE_MAX_CELLS];
+  const int cells = pa.rings * pa.sectors;
+  const int c = c0 + (int)blockIdx.y;
+  dense_place_zero(s_desc, cells);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) {
+    const float4 p = rays[i];
+    const double px = (double)p.x, py = (double)p.y, pz = (double)p.z;
+    const double len = sqrt((px * px + py * py) + pz * pz);
+    if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && len > 0.0) {
+      const double ux = px / len, uy = py / len, uz = pz / len;
+      double t;
+      const int j = dense_ray_hit(ix, cent, nrm, (double)pos[3 * c], (double)pos[3 * c + 1], (double)pos[3 * c + 2],
+                                  ux, uy, uz, a.leaf, a.min_range, a.max_range, &t);
+      if (j >= 0) {
+        const double tf = (double)(float)t;
+        unsigned b;
+        const int cell = dense_place_cell(pa, tab, (float)(tf * ux), (float)(tf * uy), (float)(tf * uz), &b);
+        if (cell >= 0) atomicMax(&s_desc[cell], b);
+      }
+    }
+  }
+  dense_place_flush(s_desc, desc + (size_t)c * cells, cells);
+}
+
+// One CTA per candidate (blockIdx.x), one thread per shift s (strided): columns j ascending, query column j against
+// candidate column (j + s) mod sectors; qq, dd and dot are fp64 sums in ascending ring; a column with qq == 0 or
+// dd == 0 is skipped, otherwise sim = dot / (sqrt(qq) * sqrt(dd)) is added; dist = 1 - sum / counted, +inf when none.
+// The best shift: smallest dist, ties to the smaller s (each thread scans its shifts ascending with a strict <, then
+// a tree over (dist, s) pairs).
+__global__ void __launch_bounds__(DENSE_PLACE_THREADS)
+dense_place_match_kernel(const unsigned* __restrict__ db, const unsigned* __restrict__ query, int rings, int sectors,
+                         double* __restrict__ best_dist, int* __restrict__ best_shift) {
+  __shared__ float s_q[DENSE_PLACE_MAX_CELLS], s_d[DENSE_PLACE_MAX_CELLS];
+  __shared__ double s_qn[DENSE_PLACE_MAX_SECTORS], s_dn[DENSE_PLACE_MAX_SECTORS];
+  __shared__ double s_bd[DENSE_PLACE_THREADS];
+  __shared__ int s_bs[DENSE_PLACE_THREADS];
+  const int cells = rings * sectors;
+  const unsigned* d = db + (size_t)blockIdx.x * cells;
+  for (int k = threadIdx.x; k < cells; k += blockDim.x) {
+    s_q[k] = __uint_as_float(__ldg(&query[k]));
+    s_d[k] = __uint_as_float(__ldg(&d[k]));
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < sectors; j += blockDim.x) {
+    double qq = 0.0, dd = 0.0;
+    for (int r = 0; r < rings; r++) {
+      const double q = (double)s_q[r * sectors + j], e = (double)s_d[r * sectors + j];
+      qq += q * q;
+      dd += e * e;
+    }
+    s_qn[j] = sqrt(qq);  // a positive sum of squares of floats is far above the smallest double: zero iff qq == 0
+    s_dn[j] = sqrt(dd);
+  }
+  __syncthreads();
+  double bd = __longlong_as_double(0x7ff0000000000000ll);
+  int bs = sectors;
+  for (int s = threadIdx.x; s < sectors; s += blockDim.x) {
+    double sum = 0.0;
+    int counted = 0;
+    for (int j = 0; j < sectors; j++) {
+      int jj = j + s;
+      if (jj >= sectors) jj -= sectors;
+      if (s_qn[j] == 0.0 || s_dn[jj] == 0.0) continue;
+      double dot = 0.0;
+      for (int r = 0; r < rings; r++) dot += (double)s_q[r * sectors + j] * (double)s_d[r * sectors + jj];
+      sum += dot / (s_qn[j] * s_dn[jj]);
+      counted++;
+    }
+    const double dist = counted ? 1.0 - sum / (double)counted : __longlong_as_double(0x7ff0000000000000ll);
+    if (dist < bd || bs == sectors) {
+      bd = dist;
+      bs = s;
+    }
+  }
+  s_bd[threadIdx.x] = bd;
+  s_bs[threadIdx.x] = bs;
+  __syncthreads();
+  for (int o = DENSE_PLACE_THREADS / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      const double d2 = s_bd[threadIdx.x + o];
+      const int s2 = s_bs[threadIdx.x + o];
+      if (d2 < s_bd[threadIdx.x] || (d2 == s_bd[threadIdx.x] && s2 < s_bs[threadIdx.x])) {
+        s_bd[threadIdx.x] = d2;
+        s_bs[threadIdx.x] = s2;
+      }
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    best_dist[blockIdx.x] = s_bd[0];
+    best_shift[blockIdx.x] = s_bs[0];
+  }
 }
 
 // ---- carve mode of the visibility pass (include/loam_b200.h "loam_b200_dense_carving")
@@ -1073,12 +1262,26 @@ struct DenseTarget {
   DevBuf<int> ray_idx;
   DevBuf<float> ray_range;        // the cast's outputs
   DevBuf<int> ray_hit;
+  // place database of loam_b200_dense_place_build: place_k descriptors of the params' cells (place_k == 0: none; a
+  // build, load or release drops it), the candidates' positions kept on the host for the global relocalisation
+  int place_k = 0;
+  DensePlaceArgs place_args{};
+  std::vector<float> place_pos;
+  DevBuf<unsigned> place_db, place_q;   // database; the query's descriptor
+  DevBuf<float> place_posd;             // positions during a build
+  DevBuf<double2> place_tab;            // sector boundaries of the call's params
+  DevBuf<double> place_dist;            // per candidate: best distance and shift of the last query
+  DevBuf<int> place_shift;
 
   void release() {
     keys.release(); keys64.release(); cent.release(); nrm.release(); pts.release(); args.release(); partials.release();
     result.release(); ticket.release(); match.release(); flag.release(); coeff.release(); sel.release();
     ray_key.release(); ray_mask.release(); ray_base.release(); ray_idx.release(); ray_range.release();
     ray_hit.release();
+    place_db.release(); place_q.release(); place_posd.release(); place_tab.release(); place_dist.release();
+    place_shift.release();
+    place_pos.clear();
+    place_k = 0;
     ray = DenseBrickIndex{};
     n = 0;
     ready = false;

@@ -299,6 +299,60 @@ void BasicLaserMapping::raycastDenseTarget(const Cloud& rays, const Twist& pose,
   if (index) index->assign(idx.begin(), idx.end());
 }
 
+static loam_b200_place_params placeParamsOf(const BasicLaserMapping::PlaceParams& p) {
+  return loam_b200_place_params{p.rings, p.sectors, p.maxRadius, p.heightOffset, p.minRange, p.maxRange};
+}
+
+void BasicLaserMapping::buildDensePlaces(const std::vector<Vector3>& positions, const Cloud& rays,
+                                         const PlaceParams& params) {
+  b200::pack(rays, _bufA);
+  std::vector<float> pos(positions.size() * 3 + 3);
+  for (size_t i = 0; i < positions.size(); i++) {
+    pos[3 * i] = positions[i].x();
+    pos[3 * i + 1] = positions[i].y();
+    pos[3 * i + 2] = positions[i].z();
+  }
+  const loam_b200_place_params prm = placeParamsOf(params);
+  _gpu->check(loam_b200_dense_place_build(_gpu->get(), pos.data(), (int)positions.size(), _bufA.data(),
+                                          (int)rays.points.size(), &prm),
+              "loam_b200_dense_place_build");
+}
+
+std::vector<BasicLaserMapping::PlaceMatch> BasicLaserMapping::queryDensePlaces(const Cloud& cloud, size_t topM) {
+  b200::pack(cloud, _bufA);
+  std::vector<loam_b200_place_match> res(topM + 1);
+  int n = 0;
+  _gpu->check(loam_b200_dense_place_query(_gpu->get(), _bufA.data(), (int)cloud.points.size(), 0, (int)topM,
+                                          res.data(), &n),
+              "loam_b200_dense_place_query");
+  std::vector<PlaceMatch> out((size_t)n);
+  for (int i = 0; i < n; i++) {
+    const loam_b200_place_match& r = res[(size_t)i];
+    out[(size_t)i] = PlaceMatch{(size_t)r.candidate, r.shift, r.yaw, Vector3(r.pos[0], r.pos[1], r.pos[2]), r.dist};
+  }
+  return out;
+}
+
+std::vector<BasicLaserMapping::RelocCandidate> BasicLaserMapping::relocalizeGlobalInDenseTarget(
+    const Cloud& cloud, const GlobalGrid& grid, const RelocParams& params, size_t maxCandidates) {
+  b200::pack(cloud, _bufA);
+  const loam_b200_reloc_params prm{params.scoreRadius, params.coarseRadius, params.fineRadius, params.keep,
+                                   params.maxIterations, params.dedupMetres, params.dedupDegrees};
+  std::vector<loam_b200_reloc_candidate> res(maxCandidates + 1);
+  int n = 0;
+  _gpu->check(loam_b200_dense_relocalize_global(_gpu->get(), _bufA.data(), (int)cloud.points.size(), 0, grid.topM,
+                                                grid.yawStepDeg, grid.yawSteps, grid.xzStep, grid.xzSteps, &prm,
+                                                res.data(), (int)maxCandidates, &n),
+              "loam_b200_dense_relocalize_global");
+  std::vector<RelocCandidate> out((size_t)n);
+  for (int i = 0; i < n; i++) {
+    const loam_b200_reloc_candidate& r = res[(size_t)i];
+    out[(size_t)i] = RelocCandidate{(size_t)r.hypothesis, (size_t)r.score_selected, toDenseAlignResult(r.coarse),
+                                    toDenseAlignResult(r.fine), (size_t)r.selected, r.rms};
+  }
+  return out;
+}
+
 std::vector<Twist> BasicLaserMapping::relocalizationGrid(const Twist& prior, float yawStepDeg, int yawSteps,
                                                          float xzStep, int xzSteps) {
   loam_b200_pose p;

@@ -760,6 +760,94 @@ int loam_b200_map_dense_raycast(void* h, const float* rays, int n, const float* 
     return 0;
   });
 }
+static loam::BasicLaserMapping::PlaceParams place_params_of(const loam_b200_place_params& p) {
+  loam::BasicLaserMapping::PlaceParams o;
+  o.rings = p.rings;
+  o.sectors = p.sectors;
+  o.maxRadius = p.max_radius;
+  o.heightOffset = p.height_offset;
+  o.minRange = p.min_range;
+  o.maxRange = p.max_range;
+  return o;
+}
+static void place_match_of(const loam::BasicLaserMapping::PlaceMatch& m, loam_b200_place_match& o) {
+  o.candidate = (int)m.candidate;
+  o.shift = m.shift;
+  o.yaw = m.yaw;
+  o.pos[0] = m.position.x(); o.pos[1] = m.position.y(); o.pos[2] = m.position.z();
+  o.dist = m.dist;
+}
+int loam_b200_map_dense_place_build(void* h, const float* positions, int k, const float* rays, int n_rays,
+                                    const loam_b200_place_params* prm) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (k < 1 || !positions || n_rays < 0 || (n_rays > 0 && !rays) || !prm) {
+    g_err = "loam_b200_map_dense_place_build: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, rays, n_rays);
+    std::vector<loam::Vector3> pos((size_t)k);
+    for (int i = 0; i < k; i++) pos[(size_t)i] = loam::Vector3(positions[3 * i], positions[3 * i + 1], positions[3 * i + 2]);
+    m->m.buildDensePlaces(pos, m->scratchA, place_params_of(*prm));
+    return 0;
+  });
+}
+int loam_b200_map_dense_place_query(void* h, const float* xyzi, int n, int top_m, loam_b200_place_match* out,
+                                    int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && !xyzi) || top_m < 1 || !out || !n_out) {
+    g_err = "loam_b200_map_dense_place_query: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, xyzi, n);
+    const auto r = m->m.queryDensePlaces(m->scratchA, (size_t)top_m);
+    *n_out = (int)r.size();
+    for (size_t i = 0; i < r.size(); i++) place_match_of(r[i], out[i]);
+    return 0;
+  });
+}
+int loam_b200_map_dense_relocalize_global(void* h, const float* xyzi, int n, int top_m, float yaw_step_deg,
+                                          int yaw_steps, float xz_step, int xz_steps,
+                                          const loam_b200_reloc_params* prm, loam_b200_reloc_candidate* out, int cap,
+                                          int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && !xyzi) || top_m < 1 || !prm || !out || cap < 1 || !n_out) {
+    g_err = "loam_b200_map_dense_relocalize_global: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, xyzi, n);
+    loam::BasicLaserMapping::RelocParams p;
+    p.scoreRadius = prm->score_radius;
+    p.coarseRadius = prm->coarse_radius;
+    p.fineRadius = prm->fine_radius;
+    p.keep = prm->keep;
+    p.maxIterations = prm->max_iterations;
+    p.dedupMetres = prm->dedup_m;
+    p.dedupDegrees = prm->dedup_deg;
+    loam::BasicLaserMapping::GlobalGrid g;
+    g.topM = top_m;
+    g.yawStepDeg = yaw_step_deg;
+    g.yawSteps = yaw_steps;
+    g.xzStep = xz_step;
+    g.xzSteps = xz_steps;
+    const auto r = m->m.relocalizeGlobalInDenseTarget(m->scratchA, g, p, (size_t)cap);
+    *n_out = (int)r.size();
+    for (size_t i = 0; i < r.size(); i++) {
+      out[i].hypothesis = (int)r[i].hypothesis;
+      out[i].score_selected = (int)r[i].scoreSelected;
+      align_result_of(r[i].coarse, out[i].coarse);
+      align_result_of(r[i].fine, out[i].fine);
+      out[i].selected = (int)r[i].selected;
+      out[i].rms = r[i].rms;
+    }
+    return 0;
+  });
+}
 int loam_b200_map_debug_dense_table_slots(void* h, long long* out) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;
   return guarded([&] { *out = ((MapH*)h)->m.denseTableSlots(); return 0; });

@@ -213,6 +213,40 @@ class BasicLaserMapping {
   // none; index (optional) its position in the target, -1 when none.
   void raycastDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& rays, const Twist& pose, float minRange,
                           float maxRange, std::vector<float>& range, std::vector<int>* index = nullptr);
+  // Place recognition and global relocalisation (include/loam_b200.h "Place recognition and global relocalisation"),
+  // for a cloud with no prior pose.  buildDensePlaces renders a polar height descriptor at each position from the
+  // target through the ray cast (rays: a sensor's directions); the database lives with the target.  queryDensePlaces
+  // compares the cloud's descriptor with every place over every heading -> the topM best, each with its heading.
+  // relocalizeGlobalInDenseTarget refines those places with relocalizeInDenseTarget over a small grid around each;
+  // a candidate's hypothesis / grid size is its place's rank.  Defaults are the recommended parameters.
+  struct PlaceParams {
+    PlaceParams() : rings(20), sectors(60), maxRadius(80.f), heightOffset(2.f), minRange(0.f), maxRange(100.f) {}
+    int rings, sectors;
+    float maxRadius, heightOffset;
+    float minRange, maxRange;  // the database's ray cast
+  };
+  struct PlaceMatch {
+    size_t candidate;  // index into the positions of buildDensePlaces
+    int shift;         // the best sector shift
+    float yaw;         // its heading (rot_y), in (-pi, pi]
+    Vector3 position;  // the place's position
+    double dist;       // descriptor distance (0: identical up to the shift)
+  };
+  struct GlobalGrid {
+    GlobalGrid() : topM(5), yawStepDeg(2.f), yawSteps(3), xzStep(0.4f), xzSteps(5) {}
+    int topM;
+    float yawStepDeg;
+    int yawSteps;
+    float xzStep;
+    int xzSteps;
+  };
+  void buildDensePlaces(const std::vector<Vector3>& positions, const pcl::PointCloud<pcl::PointXYZI>& rays,
+                        const PlaceParams& params = PlaceParams());
+  std::vector<PlaceMatch> queryDensePlaces(const pcl::PointCloud<pcl::PointXYZI>& cloud, size_t topM = 5);
+  std::vector<RelocCandidate> relocalizeGlobalInDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& cloud,
+                                                            const GlobalGrid& grid = GlobalGrid(),
+                                                            const RelocParams& params = RelocParams(),
+                                                            size_t maxCandidates = 16);
 
  private:
   typedef pcl::PointCloud<pcl::PointXYZI> Cloud;

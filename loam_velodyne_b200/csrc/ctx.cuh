@@ -278,10 +278,6 @@ struct loam_b200_ctx {
   // runs on the helper thread while the caller is back in its own code, so it is only recorded when the caller opted in
   // (loam_b200_allow_async_capture: the streaming pipeline, whose users synchronise through loam_b200_pipeline_sync).
   bool async_capture_ok = false;
-  // map_iterate_v2_kernel (persistent, warp-specialised, bulk-staged candidates): persistent grid per instantiation
-  // [store / bounding-box lookup][stage API / device loop] for the candidate capacity in use, 0 = not yet queried
-  int map_v2_grid[2][2][2] = {{{0, 0}, {0, 0}}, {{0, 0}, {0, 0}}};
-  bool map_v2_off = false;
 
   // odometry
   loamb::DevBuf<float4> od_q;  // sharp then flat

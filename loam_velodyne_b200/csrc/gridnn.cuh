@@ -162,32 +162,6 @@ __device__ __forceinline__ bool cell_in_reach(int t, float fx, float fy, float f
   return ax * ax + ay * ay + az * az <= 1.0f + 1e-5f;
 }
 
-// ---- mbarrier / bulk-copy primitives (sm_90+): one thread arms an mbarrier with the byte count it expects, any thread
-// issues cp.async.bulk copies global -> shared that complete on it; the copy engine (TMA unit, SASS UBLKCP) moves the
-// data while the issuing warps go on, and the waiters poll the barrier's phase.
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* bar, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(unsigned long long* bar, unsigned parity) {
-  unsigned ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void bulk_copy_g2s(void* dst_smem, const void* src_gmem, unsigned bytes, unsigned long long* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst_smem)),
-               "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
 // Cell lookup over the bounding-box grid of grid_build_device (kernel-level API: loam_b200_tree_build on a map slot).
 struct GridCellLookup {
   GridView g;
@@ -320,108 +294,6 @@ __device__ __forceinline__ void grid_knn5_group8(LOOKUP& lk, float qx, float qy,
     out.d[k] = bd;
     out.id[k] = bi;
     if (bi >= 0 && bi == mine.id[0]) {  // my head won: advance
-#pragma unroll
-      for (int s = 0; s < 4; s++) { mine.d[s] = mine.d[s + 1]; mine.id[s] = mine.id[s + 1]; }
-      mine.d[4] = 1.0f;
-      mine.id[4] = -1;
-    }
-  }
-}
-
-// ---- the same search with the candidate runs staged in shared memory by the copy engine ------------------------------
-// After the probes every occupied cell of the query's block is one contiguous run of 16-byte points in the cell-sorted
-// cloud.  Instead of walking the runs with per-lane loads (two in flight per lane: the kernel is latency bound), each
-// lane hands its (up to four) runs to cp.async.bulk: the whole candidate set of the query lands in `cand` (shared
-// memory, `cap` points) behind one mbarrier, then the eight
-// lanes evaluate it from shared memory.  Candidates beyond `cap` (dense maps) are still read straight from global
-// memory, so the result never depends on the capacity.  `phase` = parity of the group's mbarrier (flipped per use).
-template <typename LOOKUP>
-__device__ __forceinline__ void grid_knn5_group8_staged(LOOKUP& lk, float qx, float qy, float qz, int sub, unsigned gmask,
-                                                        unsigned* pre, unsigned* first, float4* cand, unsigned cap,
-                                                        unsigned long long* mbar, unsigned& phase, Cand5& out) {
-  Cand5 mine;
-#pragma unroll
-  for (int i = 0; i < 5; i++) { mine.d[i] = 1.0f; mine.id[i] = -1; }
-  const bool inside = lk.prepare(qx, qy, qz);
-  const float4* __restrict__ sorted = lk.points();
-  if (inside) {  // uniform over the group
-    unsigned start[4], count[4];
-    const float fx = qx - floorf(qx), fy = qy - floorf(qy), fz = qz - floorf(qz);
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const int t = sub + 8 * r;
-      start[r] = 0;
-      count[r] = 0;
-      if (t < 27 && (!lk.prune || cell_in_reach(t, fx, fy, fz))) lk.template cell<false>(t, start[r], count[r], nullptr);
-    }
-    const unsigned local = count[0] + count[1] + count[2] + count[3];
-    unsigned incl = local;
-#pragma unroll
-    for (int o = 1; o < 8; o <<= 1) {
-      const unsigned y = __shfl_up_sync(gmask, incl, o, 8);
-      if (sub >= o) incl += y;
-    }
-    const unsigned total = __shfl_sync(gmask, incl, 7, 8);
-    const unsigned staged = total < cap ? total : cap;
-    unsigned run = incl - local;
-    // the previous block's reads of `cand` (generic proxy) are ordered before the copies below (async proxy)
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      pre[sub * 4 + r] = run;
-      first[sub * 4 + r] = start[r];
-      // my run -> shared memory through the copy engine (clipped to the capacity)
-      if (count[r] > 0u && run < staged) {
-        const unsigned n_copy = (run + count[r] <= staged ? count[r] : staged - run);
-        bulk_copy_g2s(cand + run, sorted + start[r], n_copy * 16u, mbar);
-      }
-      run += count[r];
-    }
-    if (sub == 7) {
-      pre[GRID_SLOTS] = total;
-      mbar_arrive_expect_tx(mbar, staged * 16u);
-    }
-    __syncwarp(gmask);
-    const unsigned j_begin = (total * (unsigned)sub) >> 3, j_end = (total * (unsigned)(sub + 1)) >> 3;
-    // cursor of my contiguous range of the flattened list (position -> index in the sorted cloud, for ties / the fetch)
-    unsigned f = 0, hi = 0;
-    int idx = 0;
-    if (j_begin < j_end) {
-#pragma unroll
-      for (int step = 16; step > 0; step >>= 1)
-        if (pre[f + step] <= j_begin) f += step;
-      hi = pre[f + 1];
-      while (j_begin >= hi) { f++; hi = pre[f + 1]; }
-      idx = (int)(first[f] + (j_begin - pre[f]));
-    }
-    while (!mbar_try_wait(mbar, phase)) {}
-    phase ^= 1u;
-    for (unsigned j = j_begin; j < j_end; j++) {
-      const float4 p = j < staged ? cand[j] : __ldg(sorted + idx);
-      const float dx = qx - p.x, dy = qy - p.y, dz = qz - p.z;
-      cand5_offer(mine, dx * dx + dy * dy + dz * dz, idx);
-      idx++;
-      if (j + 1 < j_end && j + 1 >= hi) {
-        do { f++; hi = pre[f + 1]; } while (j + 1 >= hi);
-        idx = (int)first[f];
-      }
-    }
-  }
-  // merge the eight private lists: five rounds of "smallest head wins, winner advances"
-#pragma unroll
-  for (int k = 0; k < 5; k++) {
-    float bd = mine.d[0];
-    int bi = mine.id[0];
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) {
-      const float od = __shfl_xor_sync(gmask, bd, o);
-      const int oi = __shfl_xor_sync(gmask, bi, o);
-      const bool take = (oi >= 0) && (bi < 0 || od < bd || (od == bd && oi < bi));
-      if (take) { bd = od; bi = oi; }
-    }
-    out.d[k] = bd;
-    out.id[k] = bi;
-    if (bi >= 0 && bi == mine.id[0]) {
 #pragma unroll
       for (int s = 0; s < 4; s++) { mine.d[s] = mine.d[s + 1]; mine.id[s] = mine.id[s + 1]; }
       mine.d[4] = 1.0f;

@@ -149,20 +149,12 @@ struct StreamRunner {
   double t_reset = 0.0;  // waiting that began before the last reset of the counters is not counted
   static constexpr size_t MAX_QUEUED = 2;
 
-  // LOAM_B200_STREAM_THREADS=2: registration and odometry share one worker (two issuers + the map's helper thread contend
-  // less for the CUDA context than three; the mapping stage is the longest)
-  bool two_workers = false;
   explicit StreamRunner(PipeH* pipe) : p(pipe), device(loam::b200::defaultDevice()) {
-    if (const char* e = std::getenv("LOAM_B200_STREAM_THREADS")) two_workers = e[0] == '2';
     // users of the streaming form synchronise through loam_b200_pipeline_sync: the helper thread may record its sequence
     auto* mc = p->map.m.deviceContext();
     mc->check(loam_b200_allow_async_capture(mc->get(), 1), "loam_b200_allow_async_capture");
-    if (two_workers) {
-      th[0] = std::thread([this] { run(3); });
-    } else {
-      th[0] = std::thread([this] { run(0); });
-      th[1] = std::thread([this] { run(1); });
-    }
+    th[0] = std::thread([this] { run(0); });
+    th[1] = std::thread([this] { run(1); });
     th[2] = std::thread([this] { run(2); });
   }
   ~StreamRunner() {
@@ -202,7 +194,7 @@ struct StreamRunner {
   void run(int stage) {
     loam_b200_bind_thread(device);
     try {
-      if (stage == 0) stage_reg(); else if (stage == 1) stage_odom(); else if (stage == 2) stage_map(); else stage_reg_odom();
+      if (stage == 0) stage_reg(); else if (stage == 1) stage_odom(); else stage_map();
     } catch (const std::exception& e) {
       fail(e.what());
     } catch (...) {
@@ -232,48 +224,6 @@ struct StreamRunner {
       {
         std::lock_guard<std::mutex> lk(m);
         reg_ready = true;
-      }
-      cv.notify_all();
-    }
-  }
-  // registration + odometry of a sweep on one worker
-  void stage_reg_odom() {
-    auto& o = p->odom.o;
-    for (;;) {
-      SweepJob job;
-      const double tw = now();
-      {
-        std::unique_lock<std::mutex> lk(m);
-        wait_for(lk, [this] { return stop || !in.empty(); });
-        if (stop) return;
-        job = std::move(in.front());
-        in.pop_front();
-      }
-      cv.notify_all();
-      const double tb = now();
-      if (job.d_pts)
-        p->reg.r.processDeviceSweep(loam::Time(), job.d_pts, job.rings.data(), (int)job.rings.size());
-      else
-        p->reg.r.processPackedSweep(loam::Time(), job.pts, job.rings.data(), (int)job.rings.size());
-      const double tr = now();
-      idle[0] += tb - std::max(tw, t_reset);
-      busy[0] += tr - tb;
-      {
-        std::unique_lock<std::mutex> lk(m);
-        wait_for(lk, [this] { return stop || !odom_ready; });  // the mapping stage has taken the previous sweep over
-        if (stop) return;
-      }
-      const double ta = now();
-      o.adopt(p->reg.r);
-      const double tc = now();
-      o.process();
-      o.transformLaserCloudToEnd();
-      idle[1] += ta - tr;
-      handoff[1] += tc - ta;
-      busy[1] += now() - tc;
-      {
-        std::lock_guard<std::mutex> lk(m);
-        odom_ready = true;
       }
       cv.notify_all();
     }

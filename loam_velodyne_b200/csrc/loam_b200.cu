@@ -330,11 +330,6 @@ static void unpack_normal_eq(const float* r, loam_b200_normal_eq* out) {
   out->n_corner_selected = std::isfinite(r[28]) ? (int)(r[28] + 0.5f) : 0;
 }
 
-bool getenv_no_mailbox() {
-  static const bool off = getenv("LOAM_B200_NO_MAILBOX") != nullptr;
-  return off;
-}
-
 // mailbox of the next iteration kernel: mapped pinned memory + a fresh sequence number (mapping_lm.cuh: ResultMailbox)
 ResultMailbox next_mailbox(loam_b200_ctx* c) {
   if (c->result_mailbox.reserve(64) != cudaSuccess) {
@@ -387,7 +382,7 @@ __global__ void post_ints_kernel(const int* __restrict__ src, int n, int* host, 
 }
 
 int fetch_ints(loam_b200_ctx* c, const int* d_src, int n, int* h_dst) {
-  if (n > 500 || getenv_no_mailbox() || c->int_mailbox.reserve(512) != cudaSuccess) {
+  if (n > 500 || c->int_mailbox.reserve(512) != cudaSuccess) {
     cudaGetLastError();
     LB_CUDA(c, c->hcount.reserve(512));
     LB_CUDA(c, cudaMemcpyAsync(c->hcount.p, d_src, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -989,34 +984,6 @@ int loam_b200_map_set_queries(loam_b200_ctx* c, const float* corner, int n_corne
   return LOAM_B200_OK;
 }
 
-// map_iterate_v2_kernel: candidate capacity per query (points staged in shared memory) and the persistent grid.
-// Sparse maps (the 0.2 / 0.4 m voxel lattice of a LOAM map holds ~63 candidates per query at 1 M points) take the small
-// capacity = 4 CTAs per SM; maps beyond a few million points (~200 candidates per query) the large one.
-static int map_v2_cap_index(const loam_b200_ctx* c) {
-  const long long pts = (long long)c->cloud_n[LOAM_B200_C_MAP_CORNER_POOL] + c->cloud_n[LOAM_B200_C_MAP_SURF_POOL] +
-                        (c->map_use_store ? 0 : (long long)c->grid[0].m + c->grid[1].m);
-  return pts > 4000000 ? 1 : 0;
-}
-static const int MAP_V2_CAP[2] = {96, 224};
-extern "C++" {
-template <typename K>
-static int map_v2_grid_of(loam_b200_ctx* c, K kernel, int& cached, int cap) {
-  if (cached > 0) return cached;
-  const size_t smem = (size_t)MAP_Q_PER_BLOCK * cap * sizeof(float4);
-  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;
-  }
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, MAPV2_THREADS, smem) != cudaSuccess || per_sm < 1) {
-    cudaGetLastError();
-    return 0;
-  }
-  cached = per_sm * c->sm_count;
-  return cached;
-}
-}  // extern "C++"
-
 static int map_iterate_impl(loam_b200_ctx* c, const loam_b200_pose* pose, loam_b200_normal_eq* out, float* coeff,
                             int8_t* selected, unsigned long long* walk_totals_host = nullptr) {
   CHECK_CTX(c);
@@ -1038,8 +1005,7 @@ static int map_iterate_impl(loam_b200_ctx* c, const loam_b200_pose* pose, loam_b
   const bool dbg = coeff != nullptr;
   const ShardSpec sh = shard_spec_of(c);
   const PeerReduce pr = peer_view_of(c);
-  const bool use_mailbox = !c->comm && (c->shard_world == 1 || c->peer_ready) && !c->prof_on && !walk_totals_host &&
-                           !getenv_no_mailbox();
+  const bool use_mailbox = !c->comm && (c->shard_world == 1 || c->peer_ready) && !c->prof_on && !walk_totals_host;
   ResultMailbox mb{nullptr, 0};
   if (dbg) {
     LB_CUDA(c, c->dbg_coeff.reserve(nc + ns));
@@ -1067,32 +1033,8 @@ static int map_iterate_impl(loam_b200_ctx* c, const loam_b200_pose* pose, loam_b
     // single GPU: the folding CTA posts the sums straight into mapped host memory (no memcpy + synchronise); with a
     // shard / communicator the all-reduce has to run first, so the result is fetched the classic way
     if (use_mailbox) mb = next_mailbox(c);
-    // v2 (persistent, warp-specialised, cp.async.bulk staging) is kept as an alternative: it was slower than the
-    // phase-split kernel at config 3 -- 27 bulk copies of ~100 B per query cost more than the loads they replace.
-    // LOAM_B200_MAP_V2=1 selects it.
-    static const bool use_v2 = getenv("LOAM_B200_MAP_V2") != nullptr;
-    const int ci = map_v2_cap_index(c), cap = MAP_V2_CAP[ci];
-    int grid_v2 = 0;
-    if (use_v2 && !c->map_v2_off)
-      grid_v2 = c->map_use_store ? map_v2_grid_of(c, map_iterate_v2_kernel<MapCellLookup, false>, c->map_v2_grid[1][0][ci], cap)
-                                 : map_v2_grid_of(c, map_iterate_v2_kernel<GridCellLookup, false>, c->map_v2_grid[0][0][ci], cap);
     prof_begin(c, LOAM_B200_K_MAP_ITER);
-    if (grid_v2 > 0) {
-      const size_t smem = (size_t)MAP_Q_PER_BLOCK * cap * sizeof(float4);
-      // balanced persistent grid: every CTA gets the same number of 32-query blocks (+-1)
-      const int per_cta = (nb + grid_v2 - 1) / grid_v2;
-      const int grid = (nb + per_cta - 1) / per_cta;
-      if (c->map_use_store)
-        map_iterate_v2_kernel<MapCellLookup, false><<<grid, MAPV2_THREADS, smem, c->stream>>>(
-            store_lookup_of(c, 0), store_lookup_of(c, 1), c->map_q_corner, c->map_q_surf, nc, c0, lc, s0, ls, cb, nb, a, c->partials.p, c->result.p,
-            c->ticket.p, dbg ? c->dbg_coeff.p : nullptr, dbg ? c->dbg_sel.p : nullptr, nullptr, mb, sh, pr, cap);
-      else
-        map_iterate_v2_kernel<GridCellLookup, false><<<grid, MAPV2_THREADS, smem, c->stream>>>(
-            GridCellLookup{grid_view_of(c->grid[0])}, GridCellLookup{grid_view_of(c->grid[1])}, c->map_q_corner, c->map_q_surf, nc, c0, lc, s0, ls, cb,
-            nb, a, c->partials.p, c->result.p, c->ticket.p, dbg ? c->dbg_coeff.p : nullptr, dbg ? c->dbg_sel.p : nullptr, nullptr,
-            mb, sh, pr, cap);
-    }
-    else if (c->map_use_store)
+    if (c->map_use_store)
       map_iterate_kernel<false><<<nb, MAP_THREADS, 0, c->stream>>>(
           store_lookup_of(c, 0), store_lookup_of(c, 1), c->map_q_corner, c->map_q_surf, nc, c0, lc, s0, ls, cb, a, c->partials.p, c->result.p,
           c->ticket.p, dbg ? c->dbg_coeff.p : nullptr, dbg ? c->dbg_sel.p : nullptr, nullptr, nullptr, mb, sh, pr);
@@ -1200,7 +1142,7 @@ static int odom_iterate_impl(loam_b200_ctx* c, const loam_b200_odom_pose* pose, 
     LB_LAUNCH_CHECK(c);
   }
   ResultMailbox mb{nullptr, 0};
-  if (!c->prof_on && !getenv_no_mailbox()) mb = next_mailbox(c);
+  if (!c->prof_on) mb = next_mailbox(c);
   odom_iterate_kernel<false><<<nb, LM_THREADS, 0, c->stream>>>(view_of(tc), view_of(ts), tc.points(), ts.points(), c->od_q.p, nsh,
                                                         nfl, cb, a, c->od_ind.p, c->partials.p, c->result.p,
                                                         c->ticket.p, dbg ? c->dbg_coeff.p : nullptr,
@@ -1326,7 +1268,7 @@ int loam_b200_odom_solve(loam_b200_ctx* c, const float rot[3], const float pos[3
   LB_CUDA(c, c->partials.reserve((size_t)std::max(nb, nb_cap) * NEQ));
   LB_CUDA(c, c->lm_state.reserve(sizeof(OdomLmState) + sizeof(MapLmState)));
   OdomLmState* st = reinterpret_cast<OdomLmState*>(c->lm_state.p);
-  const bool use_mailbox = !c->prof_on && !getenv_no_mailbox() && c->result_mailbox.reserve(64) == cudaSuccess;
+  const bool use_mailbox = !c->prof_on && c->result_mailbox.reserve(64) == cudaSuccess;
   int seq = 0;
   if (use_mailbox) seq = next_mailbox(c).seq;
   OdomLoopIo io;
@@ -1419,7 +1361,7 @@ int loam_b200_map_solve(loam_b200_ctx* c, const float rot[3], const float pos[3]
   LB_CUDA(c, c->partials.reserve((size_t)std::max(nb, nb_cap) * NEQ));
   LB_CUDA(c, c->lm_state.reserve(sizeof(OdomLmState) + sizeof(MapLmState)));
   MapLmState* st = reinterpret_cast<MapLmState*>(c->lm_state.p + sizeof(OdomLmState));
-  const bool use_mailbox = use_graph && !c->prof_on && !getenv_no_mailbox() && c->result_mailbox.reserve(64) == cudaSuccess;
+  const bool use_mailbox = use_graph && !c->prof_on && c->result_mailbox.reserve(64) == cudaSuccess;
   int seq = 0;
   if (use_mailbox) seq = next_mailbox(c).seq;
   MapLoopIo io;

@@ -616,192 +616,6 @@ map_iterate_kernel(LOOKUP corner_grid, LOOKUP surf_grid, const float4* queries, 
   }
 }
 
-// ---- v2: persistent, warp-specialised, candidates staged by the copy engine -------------------------------------------
-// In the phase-split kernel above a large share of the warp samples were seven of eight warps
-// parked at the barrier while warp 0 fitted the CTA's 32 queries, and the search walked its candidate runs with two loads
-// in flight per lane (latency bound).  Here
-//   * a CTA is persistent (grid = what the GPU holds at once) and loops over blocks of 32 queries;
-//   * warps 0..7 only SEARCH (8 lanes per query), warp 8 only FITS: while warp 8 fits block i from one half of the
-//     double-buffered neighbour array, the search warps are already on block i + 1 (named barriers full / empty per half);
-//   * the candidate runs of a query are brought into shared memory by cp.async.bulk behind a per-query mbarrier
-//     (grid_knn5_group8_staged), cells out of reach are not probed at all (cell_in_reach).
-// The arithmetic per query and the order of every sum are those of map_iterate_kernel (one partial per block of 32 queries,
-// folded by the last CTA in block order), so both kernels return the same bits.
-constexpr int MAPV2_THREADS = MAP_THREADS + 32;
-__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void named_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-
-template <typename LOOKUP, bool DEVLOOP>
-__global__ void __launch_bounds__(MAPV2_THREADS, 3)
-map_iterate_v2_kernel(LOOKUP corner_grid, LOOKUP surf_grid, const float4* queries, const float4* queries_surf,
-                      int n_corner_total, int c0, int n_corner, int s0, int n_surf, int corner_blocks, int n_blocks_arg,
-                      MapIterArgs a_param,
-                      float* __restrict__ partials, float* __restrict__ result, unsigned int* ticket,
-                      float4* __restrict__ dbg_coeff, int8_t* __restrict__ dbg_sel, const MapLmState* __restrict__ lm,
-                      ResultMailbox mb, ShardSpec sh, PeerReduce pr, int cand_cap) {
-  extern __shared__ __align__(16) unsigned char smem_dyn[];
-  float4* s_cand = reinterpret_cast<float4*>(smem_dyn);  // [MAP_Q_PER_BLOCK][cand_cap]
-  __shared__ MapIterArgs s_args;
-  __shared__ alignas(16) unsigned char s_lookup[2][DEVLOOP ? MAP_LOOKUP_BYTES : 16];
-  __shared__ float4 s_nn[2][MAP_Q_PER_BLOCK][5];
-  __shared__ unsigned s_pre[MAP_Q_PER_BLOCK][GRID_SLOTS + 1];
-  __shared__ unsigned s_first[MAP_Q_PER_BLOCK][GRID_SLOTS];
-  __shared__ unsigned long long s_mbar[MAP_Q_PER_BLOCK];
-  __shared__ bool s_last;
-  int n_blocks = n_blocks_arg;
-  if (DEVLOOP) {
-    if (lm->h.done) return;
-    const MapLoopIo& io = lm->io;
-    n_blocks = io.n_blocks;
-    if (threadIdx.x < (int)(sizeof(MapIterArgs) / 4))
-      reinterpret_cast<float*>(&s_args)[threadIdx.x] = reinterpret_cast<const float*>(&lm->args)[threadIdx.x];
-    queries = io.queries; queries_surf = io.queries_surf; n_corner_total = io.n_corner_total; c0 = io.c0;
-    n_corner = io.n_corner; s0 = io.s0; n_surf = io.n_surf; corner_blocks = io.corner_blocks;
-    static_assert(sizeof(LOOKUP) <= MAP_LOOKUP_BYTES, "lookup does not fit its slot in MapLoopIo");
-    for (int w = threadIdx.x; w < 2 * (int)((sizeof(LOOKUP) + 3) / 4); w += blockDim.x) {
-      const int kind = w / (int)((sizeof(LOOKUP) + 3) / 4), k = w % (int)((sizeof(LOOKUP) + 3) / 4);
-      reinterpret_cast<unsigned*>(s_lookup[kind])[k] = reinterpret_cast<const unsigned*>(io.lookup[kind])[k];
-    }
-  }
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < MAP_Q_PER_BLOCK; i++) mbar_init(&s_mbar[i], 1u);
-    mbar_fence_init();
-    s_last = false;
-  }
-  __syncthreads();
-  const MapIterArgs& a = DEVLOOP ? s_args : a_param;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane & (MAP_GROUP - 1);
-  const unsigned gmask = 0xffu << (lane & ~(MAP_GROUP - 1));
-  const bool fit_warp = warp == MAP_THREADS / 32;
-  constexpr int BAR_FULL = 1, BAR_EMPTY = 3;  // + half (named barriers 1..4; 0 is __syncthreads)
-  unsigned mbar_phase = 0u;
-  int my_blocks = 0, it = 0;
-  for (int b = blockIdx.x; b < n_blocks; b += gridDim.x, it++) {
-    const int half = it & 1;
-    const bool is_corner = b < corner_blocks;
-    const int block_first = (is_corner ? b : b - corner_blocks) * MAP_Q_PER_BLOCK;
-    const int n_kind = is_corner ? n_corner : n_surf;
-    const int q_base = is_corner ? c0 : n_corner_total + s0;
-    const float4* __restrict__ qsrc = is_corner ? queries + c0 : queries_surf + s0;
-    if (!fit_warp) {  // ---- search warps: 8 lanes per query
-      if (it >= 2) named_bar_sync(BAR_EMPTY + half, MAPV2_THREADS);  // warp 8 is done with this half
-      LOOKUP grid = DEVLOOP ? *reinterpret_cast<const LOOKUP*>(s_lookup[is_corner ? 0 : 1]) : (is_corner ? corner_grid : surf_grid);
-      const int g = threadIdx.x / MAP_GROUP;
-      const int local = block_first + g;
-      if (local < n_kind) {  // uniform within a group of 8 lanes
-        const float4 po = qsrc[local];
-        float sx, sy, sz;
-        associate_to_map(a, po, sx, sy, sz);
-        Cand5 best;
-#pragma unroll
-        for (int i = 0; i < 5; i++) { best.d[i] = 1.0f; best.id[i] = -1; }
-        if (shard_owns(sh, store_cell(sx)))
-          grid_knn5_group8_staged(grid, sx, sy, sz, sub, gmask, s_pre[g], s_first[g], s_cand + (size_t)g * cand_cap,
-                                  (unsigned)cand_cap, &s_mbar[g], mbar_phase, best);
-        if (sub < 5) {  // lanes 0..4 fetch one neighbour each
-          const int id = sub == 0 ? best.id[0] : sub == 1 ? best.id[1] : sub == 2 ? best.id[2] : sub == 3 ? best.id[3]
-                                                                                                         : best.id[4];
-          float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (id >= 0) p = __ldg(&grid.points()[id]);
-          p.w = __int_as_float(id);
-          s_nn[half][g][sub] = p;
-        }
-      }
-      named_bar_arrive(BAR_FULL + half, MAPV2_THREADS);
-    } else {  // ---- fit warp: one query per lane
-      named_bar_sync(BAR_FULL + half, MAPV2_THREADS);
-      const int local = block_first + lane;
-      float row[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, rhs = 0.f;
-      bool sel = false;
-      if (local < n_kind) {
-        const int qi = q_base + local;
-        const float4 po = qsrc[local];
-        float sx, sy, sz;
-        associate_to_map(a, po, sx, sy, sz);
-        Top5 nn;
-#pragma unroll
-        for (int j = 0; j < 5; j++) {
-          const float4 p = s_nn[half][lane][j];
-          nn.x[j] = p.x; nn.y[j] = p.y; nn.z[j] = p.z;
-          nn.idx[j] = __float_as_int(p.w);
-          nn.d[j] = 0.f;
-        }
-        float4 coeff = make_float4(0.f, 0.f, 0.f, 0.f);
-        sel = is_corner ? corner_fit(nn, sx, sy, sz, coeff) : surf_fit(nn, sx, sy, sz, coeff);
-        if (dbg_coeff) {
-          dbg_coeff[qi] = coeff;
-          dbg_sel[qi] = sel ? 1 : 0;
-        }
-        if (sel) map_jacobian_row(a, po, coeff, row, rhs);
-      }
-      if (b + 2 * (int)gridDim.x < n_blocks) named_bar_arrive(BAR_EMPTY + half, MAPV2_THREADS);  // this half may be refilled
-      float mine = 0.f;
-      int k = 0;
-#pragma unroll
-      for (int i = 0; i < 6; i++)
-#pragma unroll
-        for (int j = i; j < 6; j++) {
-          float v = row[i] * row[j];
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-          if (lane == k) mine = v;
-          k++;
-        }
-#pragma unroll
-      for (int i = 0; i < 6; i++) {
-        float v = row[i] * rhs;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 21 + i) mine = v;
-      }
-      {
-        const unsigned sel_mask = __ballot_sync(0xffffffffu, sel);
-        if (lane == 27) mine = (float)__popc(sel_mask);
-        if (lane == 28) mine = is_corner ? (float)__popc(sel_mask) : 0.f;
-      }
-      __stcg(&partials[(size_t)b * NEQ + lane], mine);
-      my_blocks++;
-    }
-  }
-  if (fit_warp && my_blocks > 0) {
-    __threadfence();
-    __syncwarp();
-    if (lane == 0) s_last = (atomicAdd(ticket, (unsigned)my_blocks) + (unsigned)my_blocks == (unsigned)n_blocks);
-  }
-  __syncthreads();
-  if (s_last && !fit_warp) {
-    // the CTA that completed the last block folds all partials: warp w takes blocks w, w+8, ... (eight independent loads in
-    // flight) in double, then the eight warp sums are added in warp order -> run-to-run deterministic, same as v1
-    __threadfence();
-    __shared__ double s_fold[MAP_THREADS / 32][NEQ];
-    constexpr unsigned NW = MAP_THREADS / 32;
-    const unsigned nb = (unsigned)n_blocks;
-    double v = 0.0;
-    unsigned bk = warp;
-    for (; bk + 7 * NW < nb; bk += 8 * NW) {
-      float t[8];
-#pragma unroll
-      for (int u = 0; u < 8; u++) t[u] = __ldcg(&partials[(size_t)(bk + u * NW) * NEQ + lane]);
-#pragma unroll
-      for (int u = 0; u < 8; u++) v += (double)t[u];
-    }
-    for (; bk < nb; bk += NW) v += (double)__ldcg(&partials[(size_t)bk * NEQ + lane]);
-    s_fold[warp][lane] = v;
-    named_bar_sync(5, MAP_THREADS);  // the eight folding warps only
-    if (threadIdx.x < NEQ) {
-      double r = 0.0;
-      for (unsigned wv = 0; wv < NW; wv++) r += s_fold[wv][threadIdx.x];
-      float rf = (float)r;
-      if (pr.world > 1) rf = peer_allreduce32<0>(pr, rf);  // fused all-reduce over NVLink peer memory (warp 0)
-      result[threadIdx.x] = rf;
-      mailbox_post_value(mb, threadIdx.x, rf);
-    }
-    if (threadIdx.x == 0) *ticket = 0u;
-    named_bar_sync(5, MAP_THREADS);
-    mailbox_post_seq(mb);
-  }
-}
-
 __global__ void map_lm_step_kernel(MapLmState* st, const float* __restrict__ result, unsigned long long handle = 0ull,
                                    float* mailbox_host = nullptr) {
   __shared__ float s_r[NEQ];  // see odom_lm_step_kernel

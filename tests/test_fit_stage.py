@@ -1,16 +1,11 @@
 """Every compiled copy of the per-correspondence line and plane fits against the fp32 restatement of
 tests/fit_reference.py (pinned to the checker by test_fit_reference.py), bit for bit and NaN-aware, with no slack:
-map_iterate_kernel and map_iterate_v2_kernel, each over the bounding-box grid (GridCellLookup) and the pipeline's
-persistent store (MapCellLookup), and the odometry iteration kernel through both of its entry paths.  The inputs are
+map_iterate_kernel over the bounding-box grid (GridCellLookup) and over the pipeline's persistent store
+(MapCellLookup), and the odometry iteration kernel through both of its entry paths.  The inputs are
 the catalogue of degenerate neighbourhoods of fit_reference.cases / odom_cases and the real sweeps of the existing
 per-correspondence tests, restricted there to queries whose search has no exact distance tie."""
 import contextlib
-import json
 import math
-import os
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -21,7 +16,6 @@ from test_fit_reference import (TWIST, YAW, ZERO, batch_clouds, batches, check_o
                                 odom_restate_ind, odom_rows, odom_sweep, restate)
 
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
 LEAVES = (0.2, 0.4)
 
 
@@ -144,28 +138,6 @@ def store_checks(oracle, catalogue):
 def test_store_path_catalogue(oracle):
     cat = fr.cases(0, oracle)
     assert store_checks(oracle, cat) == len([c for c in cat if c.batch != "far"]) + len(fr.tie_cases())
-
-
-# ---------------------------------------------------------------------------------------------- mapping: v2 kernel
-def _v2_main(out):
-    """Child-process body of test_v2_kernel_catalogue (LOAM_B200_MAP_V2 is read once per process)."""
-    import __graft_entry__  # noqa: F401  (puts the repository root on sys.path)
-    from oracle import pydriver
-    oracle = pydriver.load("restatement")
-    cat = fr.cases(0, oracle)
-    n = grid_checks(oracle, cat, ["zero", "yaw"]) + store_checks(oracle, cat)
-    json.dump({"n": n}, open(out, "w"))
-
-
-def test_v2_kernel_catalogue(oracle):
-    with tempfile.TemporaryDirectory() as tmp:
-        out = os.path.join(tmp, "out.json")
-        env = dict(os.environ, LOAM_B200_MAP_V2="1")
-        env["PYTHONPATH"] = os.pathsep.join([HERE, os.path.dirname(HERE), env.get("PYTHONPATH", "")])
-        r = subprocess.run([sys.executable, "-c", "import sys, test_fit_stage as t; t._v2_main(sys.argv[1])", out],
-                           capture_output=True, text=True, timeout=900, env=env, cwd=HERE)
-        assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-5000:]
-        assert json.load(open(out))["n"] > 200
 
 
 # ---------------------------------------------------------------------------------------------- odometry

@@ -40,6 +40,9 @@ static int async_join(loam_b200_ctx* c, bool order = true);
 
 namespace {
 
+// cloud slot of the persistent map pool of each kind (0 corner, 1 surface)
+const int POOL_SLOT[2] = {LOAM_B200_C_MAP_CORNER_POOL, LOAM_B200_C_MAP_SURF_POOL};
+
 inline int blocks_for(long long n, int bs) { return (int)((n + bs - 1) / bs); }
 
 TreeView view_of(const Tree& t) {
@@ -135,13 +138,59 @@ GridView grid_view_of(const Grid& g) {
 MapCellLookup store_lookup_of(const loam_b200_ctx* c, int kind) {
   const auto& st = c->store[kind];
   MapCellLookup lk;
-  lk.g = MapGridView{st.table.p, st.mask, c->cloud[kind == 0 ? LOAM_B200_C_MAP_CORNER_POOL : LOAM_B200_C_MAP_SURF_POOL].p,
-                     c->rank_of_cube.p, c->map_grid.cen_w, c->map_grid.cen_h, c->map_grid.cen_d, c->map_n_valid};
+  lk.g = MapGridView{st.table.p, st.mask, c->cloud[POOL_SLOT[kind]].p, c->rank_of_cube.p, c->map_grid.cen_w,
+                     c->map_grid.cen_h, c->map_grid.cen_d, c->map_n_valid};
   lk.ax = lk.ay = lk.az = CellAxis{0, 0, 0};
   // maps whose points (16 B each) take more than half of L2 are fetched from HBM: prune the unreachable cells there
   const long long map_pts = (long long)c->cloud_n[LOAM_B200_C_MAP_CORNER_POOL] + c->cloud_n[LOAM_B200_C_MAP_SURF_POOL];
   lk.prune = c->map_prune_mode >= 0 ? c->map_prune_mode : (map_pts * 16 > (long long)c->l2_bytes / 2 ? 1 : 0);
   return lk;
+}
+
+// `f(corner, surf)` on the scan-to-map search structure: the persistent cell-sorted pools (stage API) or the grids over
+// the two map slots (kernel-level API)
+template <typename F>
+void with_map_lookups(const loam_b200_ctx* c, F f) {
+  if (c->map_use_store)
+    f(store_lookup_of(c, 0), store_lookup_of(c, 1));
+  else
+    f(GridCellLookup{grid_view_of(c->grid[0])}, GridCellLookup{grid_view_of(c->grid[1])});
+}
+
+// blocks of an iteration kernel over n_a + n_b queries (two query kinds, `per_block` queries per block; at least one)
+int lm_blocks(int n_a, int n_b, int per_block) {
+  return std::max(blocks_for(n_a, per_block) + blocks_for(n_b, per_block), 1);
+}
+
+// This rank's contiguous slice of each scan-to-map query kind, [c0, c0 + lc) and [s0, s0 + ls), and the iteration
+// kernel's grid over it: everything when not sharded, and with the cube-sharded map (shard_slab > 0), where every rank
+// looks at every query and evaluates those whose transformed position falls into a cell it owns.
+struct MapSlice { int c0, lc, s0, ls, cb, nb; };
+MapSlice map_slice_of(const loam_b200_ctx* c) {
+  const int nc = c->map_nc, ns = c->map_ns;
+  const int W = c->shard_slab > 0 ? 1 : c->shard_world, R = c->shard_slab > 0 ? 0 : c->shard_rank;
+  MapSlice q;
+  q.c0 = (int)((long long)nc * R / W);
+  q.lc = (int)((long long)nc * (R + 1) / W) - q.c0;
+  q.s0 = (int)((long long)ns * R / W);
+  q.ls = (int)((long long)ns * (R + 1) / W) - q.s0;
+  q.cb = blocks_for(q.lc, MAP_Q_PER_BLOCK);
+  q.nb = lm_blocks(q.lc, q.ls, MAP_Q_PER_BLOCK);
+  return q;
+}
+
+// The one launch of the scan-to-map iteration kernel, on c->map_q_* and the lookups of c->map_use_store.  STATS counts
+// the search's walk into walk_totals; DEVLOOP takes slice, arguments and lookups from the loop's state block `lm`.
+template <bool STATS, bool DEVLOOP>
+void launch_map_iterate(loam_b200_ctx* c, int grid, const MapSlice& q, const MapIterArgs& a, float4* dbg_coeff,
+                        int8_t* dbg_sel, unsigned long long* walk_totals, const MapLmState* lm = nullptr,
+                        ResultMailbox mb = ResultMailbox{nullptr, 0}, ShardSpec sh = ShardSpec{0, 1, 0},
+                        PeerReduce pr = PeerReduce{}) {
+  with_map_lookups(c, [&](auto corner, auto surf) {
+    map_iterate_kernel<STATS, decltype(corner), DEVLOOP><<<grid, MAP_THREADS, 0, c->stream>>>(
+        corner, surf, c->map_q_corner, c->map_q_surf, c->map_nc, q.c0, q.lc, q.s0, q.ls, q.cb, a, c->partials.p,
+        c->result.p, c->ticket.p, dbg_coeff, dbg_sel, walk_totals, lm, mb, sh, pr);
+  });
 }
 
 // 1 m uniform grid over d_pts: the search structure of the scan-to-map loop (gridnn.cuh).  m is the launch bound; when
@@ -340,21 +389,27 @@ ResultMailbox next_mailbox(loam_b200_ctx* c) {
   return ResultMailbox{c->result_mailbox.p, c->result_seq};
 }
 
-// wait for the kernel launched with next_mailbox() to post its sums; falls back to a stream synchronise (which also
-// surfaces launch failures) when nothing arrives for a long time
-int fetch_normal_eq_mailbox(loam_b200_ctx* c, loam_b200_normal_eq* out) {
-  volatile int* seq = reinterpret_cast<volatile int*>(c->result_mailbox.p + 32);
+// wait until a kernel posts `expected` into the sequence word of a mapped host mailbox; falls back to a stream
+// synchronise (which also surfaces launch failures) when nothing arrives for 2 s.  The payload is readable on return.
+static int wait_mailbox(loam_b200_ctx* c, const volatile int* seq, int expected) {
   const auto t0 = std::chrono::steady_clock::now();
   long long spins = 0;
-  while (*seq != c->result_seq) {
+  while (*seq != expected) {
     if ((++spins & 0xfff) == 0 &&
         std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > 2.0) {
       LB_CUDA(c, cudaStreamSynchronize(c->stream));  // error or a very long kernel: by now the post is visible
-      if (*seq != c->result_seq) return LOAM_B200_ERR_CUDA;
+      if (*seq != expected) return LOAM_B200_ERR_CUDA;
       break;
     }
   }
   std::atomic_thread_fence(std::memory_order_acquire);
+  return LOAM_B200_OK;
+}
+
+// the sums of the kernel launched with next_mailbox()
+int fetch_normal_eq_mailbox(loam_b200_ctx* c, loam_b200_normal_eq* out) {
+  const int rc = wait_mailbox(c, reinterpret_cast<volatile int*>(c->result_mailbox.p + 32), c->result_seq);
+  if (rc) return rc;
   float r[NEQ];
   for (int i = 0; i < NEQ; i++) r[i] = reinterpret_cast<volatile float*>(c->result_mailbox.p)[i];
   unpack_normal_eq(r, out);
@@ -366,6 +421,21 @@ int fetch_normal_eq(loam_b200_ctx* c, loam_b200_normal_eq* out) {
   LB_CUDA(c, cudaMemcpyAsync(c->result_host.p, c->result.p, NEQ * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   LB_CUDA(c, cudaStreamSynchronize(c->stream));
   unpack_normal_eq(c->result_host.p, out);
+  return LOAM_B200_OK;
+}
+
+// The end of one per-iteration call over n queries: the sums (from the mailbox when the kernel posted there), then in
+// debug mode (coeff given) the per-query outputs the kernel wrote, `ind` only for the odometry.
+int finish_iteration(loam_b200_ctx* c, const ResultMailbox& mb, loam_b200_normal_eq* out, int n, float* coeff,
+                     int8_t* selected, int32_t* ind) {
+  const int rc = mb.host ? fetch_normal_eq_mailbox(c, out) : fetch_normal_eq(c, out);
+  if (rc) return rc;
+  if (coeff) {
+    LB_CUDA(c, cudaMemcpyAsync(coeff, c->dbg_coeff.p, (size_t)n * 16, cudaMemcpyDeviceToHost, c->stream));
+    if (selected) LB_CUDA(c, cudaMemcpyAsync(selected, c->dbg_sel.p, (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+    if (ind) LB_CUDA(c, cudaMemcpyAsync(ind, c->od_ind.p, (size_t)n * 3 * 4, cudaMemcpyDeviceToHost, c->stream));
+    LB_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
   return LOAM_B200_OK;
 }
 
@@ -393,17 +463,8 @@ int fetch_ints(loam_b200_ctx* c, const int* d_src, int n, int* h_dst) {
   c->int_seq = c->int_seq == 0x7fffffff ? 1 : c->int_seq + 1;
   post_ints_kernel<<<1, 32, 0, c->stream>>>(d_src, n, c->int_mailbox.p, c->int_seq);
   LB_LAUNCH_CHECK(c);
-  volatile int* seq = reinterpret_cast<volatile int*>(c->int_mailbox.p + 511);
-  const auto t0 = std::chrono::steady_clock::now();
-  long long spins = 0;
-  while (*seq != c->int_seq) {
-    if ((++spins & 0xfff) == 0 && std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > 2.0) {
-      LB_CUDA(c, cudaStreamSynchronize(c->stream));
-      if (*seq != c->int_seq) return LOAM_B200_ERR_CUDA;
-      break;
-    }
-  }
-  std::atomic_thread_fence(std::memory_order_acquire);
+  const int rc = wait_mailbox(c, reinterpret_cast<volatile int*>(c->int_mailbox.p + 511), c->int_seq);
+  if (rc) return rc;
   for (int i = 0; i < n; i++) h_dst[i] = reinterpret_cast<volatile int*>(c->int_mailbox.p)[i];
   return LOAM_B200_OK;
 }
@@ -993,18 +1054,11 @@ static int map_iterate_impl(loam_b200_ctx* c, const loam_b200_pose* pose, loam_b
   if (nc + ns == 0) return LOAM_B200_OK;
   MapIterArgs a;
   fill_map_args(pose, a);
-  // this rank's contiguous slice of each query kind (everything when not sharded, and with the cube-sharded map, where
-  // every rank looks at every query and evaluates those whose transformed position falls into a cell it owns)
-  const int W = c->shard_slab > 0 ? 1 : c->shard_world, R = c->shard_slab > 0 ? 0 : c->shard_rank;
-  const int c0 = (int)((long long)nc * R / W), c1 = (int)((long long)nc * (R + 1) / W);
-  const int s0 = (int)((long long)ns * R / W), s1 = (int)((long long)ns * (R + 1) / W);
-  const int lc = c1 - c0, ls = s1 - s0;
-  const int cb = blocks_for(lc, MAP_Q_PER_BLOCK), sb = blocks_for(ls, MAP_Q_PER_BLOCK);
-  const int nb = std::max(cb + sb, 1);
-  LB_CUDA(c, c->partials.reserve((size_t)nb * NEQ));
+  const MapSlice q = map_slice_of(c);
+  LB_CUDA(c, c->partials.reserve((size_t)q.nb * NEQ));
   const bool dbg = coeff != nullptr;
-  const ShardSpec sh = shard_spec_of(c);
-  const PeerReduce pr = peer_view_of(c);
+  // single GPU: the folding CTA posts the sums straight into mapped host memory (no memcpy + synchronise); with a
+  // shard / communicator the all-reduce has to run first, so the result is fetched the classic way
   const bool use_mailbox = !c->comm && (c->shard_world == 1 || c->peer_ready) && !c->prof_on && !walk_totals_host;
   ResultMailbox mb{nullptr, 0};
   if (dbg) {
@@ -1018,31 +1072,15 @@ static int map_iterate_impl(loam_b200_ctx* c, const loam_b200_pose* pose, loam_b
   if (walk_totals_host) {
     LB_CUDA(c, c->walk_totals.reserve(2));
     LB_CUDA(c, cudaMemsetAsync(c->walk_totals.p, 0, 2 * sizeof(unsigned long long), c->stream));
-    if (c->map_use_store)
-      map_iterate_kernel<true><<<nb, MAP_THREADS, 0, c->stream>>>(
-          store_lookup_of(c, 0), store_lookup_of(c, 1), c->map_q_corner, c->map_q_surf, nc, c0, lc, s0, ls, cb, a, c->partials.p, c->result.p,
-          c->ticket.p, nullptr, nullptr, c->walk_totals.p);
-    else
-      map_iterate_kernel<true><<<nb, MAP_THREADS, 0, c->stream>>>(
-          GridCellLookup{grid_view_of(c->grid[0])}, GridCellLookup{grid_view_of(c->grid[1])}, c->map_q_corner, c->map_q_surf, nc, c0, lc, s0, ls,
-          cb, a, c->partials.p, c->result.p, c->ticket.p, nullptr, nullptr, c->walk_totals.p);
+    launch_map_iterate<true, false>(c, q.nb, q, a, nullptr, nullptr, c->walk_totals.p);
     LB_LAUNCH_CHECK(c);
     LB_CUDA(c, cudaMemcpyAsync(walk_totals_host, c->walk_totals.p, 2 * sizeof(unsigned long long),
                                cudaMemcpyDeviceToHost, c->stream));
   } else {
-    // single GPU: the folding CTA posts the sums straight into mapped host memory (no memcpy + synchronise); with a
-    // shard / communicator the all-reduce has to run first, so the result is fetched the classic way
     if (use_mailbox) mb = next_mailbox(c);
     prof_begin(c, LOAM_B200_K_MAP_ITER);
-    if (c->map_use_store)
-      map_iterate_kernel<false><<<nb, MAP_THREADS, 0, c->stream>>>(
-          store_lookup_of(c, 0), store_lookup_of(c, 1), c->map_q_corner, c->map_q_surf, nc, c0, lc, s0, ls, cb, a, c->partials.p, c->result.p,
-          c->ticket.p, dbg ? c->dbg_coeff.p : nullptr, dbg ? c->dbg_sel.p : nullptr, nullptr, nullptr, mb, sh, pr);
-    else
-      map_iterate_kernel<false><<<nb, MAP_THREADS, 0, c->stream>>>(
-          GridCellLookup{grid_view_of(c->grid[0])}, GridCellLookup{grid_view_of(c->grid[1])}, c->map_q_corner, c->map_q_surf, nc, c0, lc, s0, ls,
-          cb, a, c->partials.p, c->result.p, c->ticket.p, dbg ? c->dbg_coeff.p : nullptr, dbg ? c->dbg_sel.p : nullptr,
-          nullptr, nullptr, mb, sh, pr);
+    launch_map_iterate<false, false>(c, q.nb, q, a, dbg ? c->dbg_coeff.p : nullptr, dbg ? c->dbg_sel.p : nullptr,
+                                     nullptr, nullptr, mb, shard_spec_of(c), peer_view_of(c));
     LB_LAUNCH_CHECK(c);
     prof_end(c);
   }
@@ -1050,18 +1088,12 @@ static int map_iterate_impl(loam_b200_ctx* c, const loam_b200_pose* pose, loam_b
     const int rcc = allreduce_result(c);  // no-op without a communicator
     if (rcc) return rcc;
   }
-  int rc = mb.host ? fetch_normal_eq_mailbox(c, out) : fetch_normal_eq(c, out);
+  const int rc = finish_iteration(c, mb, out, nc + ns, coeff, selected, nullptr);
   if (rc) return rc;
   if (c->peer_ready && c->shard_world > 1 && !std::isfinite(out->AtB[0] + out->AtA[0])) {
     // the fused all-reduce gives up (NaN sums) when a peer's contribution does not arrive within ~2 s
     c->last_error = "peer all-reduce timed out: a rank of the cube-sharded map did not run this iteration";
     return LOAM_B200_ERR_COMM;
-  }
-  if (dbg) {
-    LB_CUDA(c, cudaMemcpyAsync(coeff, c->dbg_coeff.p, (size_t)(nc + ns) * 16, cudaMemcpyDeviceToHost, c->stream));
-    if (selected)
-      LB_CUDA(c, cudaMemcpyAsync(selected, c->dbg_sel.p, (size_t)(nc + ns), cudaMemcpyDeviceToHost, c->stream));
-    LB_CUDA(c, cudaStreamSynchronize(c->stream));
   }
   return LOAM_B200_OK;
 }
@@ -1141,25 +1173,16 @@ static int odom_iterate_impl(loam_b200_ctx* c, const loam_b200_odom_pose* pose, 
         ring_off_search(c, 0), ring_off_search(c, 1));
     LB_LAUNCH_CHECK(c);
   }
+  const bool use_mailbox = !c->prof_on;
   ResultMailbox mb{nullptr, 0};
-  if (!c->prof_on) mb = next_mailbox(c);
+  if (use_mailbox) mb = next_mailbox(c);
   odom_iterate_kernel<false><<<nb, LM_THREADS, 0, c->stream>>>(view_of(tc), view_of(ts), tc.points(), ts.points(), c->od_q.p, nsh,
                                                         nfl, cb, a, c->od_ind.p, c->partials.p, c->result.p,
                                                         c->ticket.p, dbg ? c->dbg_coeff.p : nullptr,
                                                         dbg ? c->dbg_sel.p : nullptr, nullptr, mb);
   LB_LAUNCH_CHECK(c);
   prof_end(c);
-  int rc = mb.host ? fetch_normal_eq_mailbox(c, out) : fetch_normal_eq(c, out);
-  if (rc) return rc;
-  if (dbg) {
-    LB_CUDA(c, cudaMemcpyAsync(coeff, c->dbg_coeff.p, (size_t)(nsh + nfl) * 16, cudaMemcpyDeviceToHost, c->stream));
-    if (selected)
-      LB_CUDA(c, cudaMemcpyAsync(selected, c->dbg_sel.p, (size_t)(nsh + nfl), cudaMemcpyDeviceToHost, c->stream));
-    if (ind)
-      LB_CUDA(c, cudaMemcpyAsync(ind, c->od_ind.p, (size_t)(nsh + nfl) * 3 * 4, cudaMemcpyDeviceToHost, c->stream));
-    LB_CUDA(c, cudaStreamSynchronize(c->stream));
-  }
-  return LOAM_B200_OK;
+  return finish_iteration(c, mb, out, nsh + nfl, coeff, selected, ind);
 }
 
 int loam_b200_odom_iterate(loam_b200_ctx* c, const loam_b200_odom_pose* pose, loam_b200_normal_eq* out) {
@@ -1188,19 +1211,11 @@ static int lm_read_header(loam_b200_ctx* c, const void* d_state, LmHeader* h) {
   return LOAM_B200_OK;
 }
 
-// wait for the loop's final header in the mailbox (see fetch_normal_eq_mailbox)
+// the loop's final header in the mailbox (lmstep.cuh: lm_loop_control)
 static int lm_wait_mailbox(loam_b200_ctx* c, LmHeader* h) {
   volatile int* box = reinterpret_cast<volatile int*>(c->result_mailbox.p);
-  const auto t0 = std::chrono::steady_clock::now();
-  long long spins = 0;
-  while (box[32] != c->result_seq) {
-    if ((++spins & 0xfff) == 0 && std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > 2.0) {
-      LB_CUDA(c, cudaStreamSynchronize(c->stream));
-      if (box[32] != c->result_seq) return LOAM_B200_ERR_CUDA;
-      break;
-    }
-  }
-  std::atomic_thread_fence(std::memory_order_acquire);
+  const int rc = wait_mailbox(c, box + 32, c->result_seq);
+  if (rc) return rc;
   int* w = reinterpret_cast<int*>(h);
   for (int i = 0; i < 9; i++) w[i] = box[i];
   return LOAM_B200_OK;
@@ -1208,8 +1223,18 @@ static int lm_wait_mailbox(loam_b200_ctx* c, LmHeader* h) {
 
 static int round_cap(int n) { return ((n + n / 4 + 255) / 256) * 256; }  // 25 % head room, multiples of 256 queries
 
-// (re)build a loop graph: `launch_gate` and `launch_body` enqueue their kernels on c->stream (captured, not run)
+static bool loop_graphs_enabled() {
+  static const bool off = getenv("LOAM_B200_NO_LOOP_GRAPH") != nullptr;
+  return !off;
+}
+
+// per_block: queries per block of the iteration kernel; kernels_per_iter: launched by the WHILE body per executed
+// iteration; chunk: iterations between header reads without a graph; variant: kernel instantiation in the graph body;
+// reduce: all-reduce the sums between iteration kernels and step (communicator only, which rules out the graph)
+struct LmLoopShape { int per_block, kernels_per_iter, chunk, variant; bool reduce; int prof_family; };
+
 extern "C++" {
+// (re)build a loop graph: `launch_gate` and `launch_body` enqueue their kernels on c->stream (captured, not run)
 template <typename GATE, typename BODY>
 static int loop_graph_build(loam_b200_ctx* c, LoopGraph& lg, GATE launch_gate, BODY launch_body) {
   lg.destroy();
@@ -1239,12 +1264,71 @@ static int loop_graph_build(loam_b200_ctx* c, LoopGraph& lg, GATE launch_gate, B
   lg.builds++;
   return LOAM_B200_OK;
 }
-}  // extern "C++"
 
-static bool loop_graphs_enabled() {
-  static const bool off = getenv("LOAM_B200_NO_LOOP_GRAPH") != nullptr;
-  return !off;
+// One device-resident loop over n_a + n_b queries on the state block headed by `hdr`.  The stage's launchers neither
+// check nor count: launch_init(mailbox seq or 0), launch_iter(it, q_a, q_b, grid) -> kernels launched (the graph body
+// is captured once with it = 0 and the capacities; its kernels read the iteration from the state block), and
+// launch_step(condition handle, mailbox) (0, nullptr outside a graph).
+template <typename INIT, typename ITER, typename STEP>
+static int lm_loop_solve(loam_b200_ctx* c, LoopGraph& lg, LmHeader* hdr, const LmLoopShape& s, int n_a, int n_b,
+                         int max_iterations, INIT launch_init, ITER launch_iter, STEP launch_step,
+                         loam_b200_lm_result* out) {
+  const bool use_graph = loop_graphs_enabled() && !(s.reduce && c->comm);
+  const int cap_a = use_graph ? std::max(lg.cap_a, n_a > lg.cap_a ? round_cap(n_a) : 0) : n_a;
+  const int cap_b = use_graph ? std::max(lg.cap_b, n_b > lg.cap_b ? round_cap(n_b) : 0) : n_b;
+  const int nb = lm_blocks(n_a, n_b, s.per_block), nb_cap = lm_blocks(cap_a, cap_b, s.per_block);
+  LB_CUDA(c, c->partials.reserve((size_t)std::max(nb, nb_cap) * NEQ));
+  const bool use_mailbox = use_graph && !c->prof_on && c->result_mailbox.reserve(64) == cudaSuccess;
+  launch_init(use_mailbox ? next_mailbox(c).seq : 0);
+  LB_LAUNCH_CHECK(c);
+  LmHeader h{};
+  prof_begin(c, s.prof_family);
+  if (use_graph) {
+    const void* baked[4] = {hdr, c->partials.p, c->result.p, use_mailbox ? (void*)c->result_mailbox.p : nullptr};
+    if (!lg.exec || lg.cap_a != cap_a || lg.cap_b != cap_b || lg.variant != s.variant ||
+        memcmp(lg.baked, baked, sizeof baked) != 0) {
+      float* mbp = use_mailbox ? c->result_mailbox.p : nullptr;
+      unsigned long long* hp = &lg.handle;
+      const int rc = loop_graph_build(
+          c, lg, [&] { lm_gate_kernel<<<1, 32, 0, c->stream>>>(hdr, *hp, mbp); },
+          [&] {
+            launch_iter(0, cap_a, cap_b, nb_cap);
+            launch_step(*hp, mbp);
+          });
+      if (rc) return rc;
+      lg.cap_a = cap_a; lg.cap_b = cap_b; lg.variant = s.variant;
+      memcpy(lg.baked, baked, sizeof baked);
+    }
+    LB_CUDA(c, cudaGraphLaunch(lg.exec, c->stream));
+    const int rc = use_mailbox ? lm_wait_mailbox(c, &h) : lm_read_header(c, hdr, &h);
+    if (rc) return rc;
+    // gate + the kernels of every executed iteration, launched by the WHILE node
+    c->launches += 1 + s.kernels_per_iter * h.iters_run;
+    g_total_launches.fetch_add(1 + s.kernels_per_iter * h.iters_run, std::memory_order_relaxed);
+  } else {
+    for (int it = 0; it < max_iterations;) {
+      const int chunk_end = std::min(max_iterations, it + s.chunk);
+      for (; it < chunk_end; it++) {
+        for (int k = launch_iter(it, n_a, n_b, nb); k > 0; k--) LB_LAUNCH_CHECK(c);
+        if (s.reduce) {
+          const int rcc = allreduce_result(c);  // every rank then takes the same step
+          if (rcc) return rcc;
+        }
+        launch_step(0ull, nullptr);
+        LB_LAUNCH_CHECK(c);
+      }
+      const int rc = lm_read_header(c, hdr, &h);
+      if (rc) return rc;
+      if (h.done) break;
+    }
+  }
+  prof_end(c);
+  for (int i = 0; i < 3; i++) { out->rot[i] = h.rot[i]; out->pos[i] = h.pos[i]; }
+  out->iterations = h.iters_run;
+  out->converged = h.done ? 1 : 0;
+  return LOAM_B200_OK;
 }
+}  // extern "C++"
 
 int loam_b200_odom_solve(loam_b200_ctx* c, const float rot[3], const float pos[3], float inv_scan_period, int max_iterations,
                          float delta_t_abort, float delta_r_abort, loam_b200_lm_result* out) {
@@ -1258,185 +1342,81 @@ int loam_b200_odom_solve(loam_b200_ctx* c, const float rot[3], const float pos[3
   if (nsh + nfl == 0 || max_iterations == 0) return LOAM_B200_OK;
   const Tree& tc = c->tree[LOAM_B200_TREE_ODOM_CORNER];
   const Tree& ts = c->tree[LOAM_B200_TREE_ODOM_SURF];
-  const bool use_graph = loop_graphs_enabled();
-  LoopGraph& lg = c->odom_loop;
-  const int cap_sh = use_graph ? std::max(lg.cap_a, nsh > lg.cap_a ? round_cap(nsh) : 0) : nsh;
-  const int cap_fl = use_graph ? std::max(lg.cap_b, nfl > lg.cap_b ? round_cap(nfl) : 0) : nfl;
-  const int cb = blocks_for(nsh, LM_THREADS), sb = blocks_for(nfl, LM_THREADS);
-  const int nb = cb + sb;
-  const int nb_cap = blocks_for(cap_sh, LM_THREADS) + blocks_for(cap_fl, LM_THREADS);
-  LB_CUDA(c, c->partials.reserve((size_t)std::max(nb, nb_cap) * NEQ));
   LB_CUDA(c, c->lm_state.reserve(sizeof(OdomLmState) + sizeof(MapLmState)));
   OdomLmState* st = reinterpret_cast<OdomLmState*>(c->lm_state.p);
-  const bool use_mailbox = !c->prof_on && c->result_mailbox.reserve(64) == cudaSuccess;
-  int seq = 0;
-  if (use_mailbox) seq = next_mailbox(c).seq;
   OdomLoopIo io;
   io.corner_tree = view_of(tc); io.surf_tree = view_of(ts);
   io.last_corner = tc.points(); io.last_surf = ts.points(); io.queries = c->od_q.p; io.ind = c->od_ind.p;
   io.ring_off_corner = ring_off_search(c, 0); io.ring_off_surf = ring_off_search(c, 1);
-  io.n_sharp = nsh; io.n_flat = nfl; io.sharp_blocks = cb; io.n_blocks = nb;
-  odom_lm_init_kernel<<<1, 32, 0, c->stream>>>(st, rot[0], rot[1], rot[2], pos[0], pos[1], pos[2], inv_scan_period,
-                                               delta_t_abort, delta_r_abort, max_iterations, tc.m, ts.m, io, seq);
-  LB_LAUNCH_CHECK(c);
+  io.n_sharp = nsh; io.n_flat = nfl; io.sharp_blocks = blocks_for(nsh, LM_THREADS);
+  io.n_blocks = lm_blocks(nsh, nfl, LM_THREADS);
   const OdomIterArgs unused{};
   const TreeView tv0{};
-  LmHeader h{};
-  prof_begin(c, LOAM_B200_K_ODOM_ITER);
-  if (use_graph) {
-    const void* baked[4] = {st, c->partials.p, c->result.p, use_mailbox ? (void*)c->result_mailbox.p : nullptr};
-    if (!lg.exec || lg.cap_a != cap_sh || lg.cap_b != cap_fl || memcmp(lg.baked, baked, sizeof baked) != 0) {
-      float* mbp = use_mailbox ? c->result_mailbox.p : nullptr;
-      unsigned long long* hp = &lg.handle;
-      const int rc = loop_graph_build(
-          c, lg, [&] { lm_gate_kernel<<<1, 32, 0, c->stream>>>(&st->h, *hp, mbp); },
-          [&] {
-            odom_search_kernel<true><<<blocks_for((long long)(cap_sh + cap_fl) * 32, LM_THREADS), LM_THREADS, 0, c->stream>>>(
-                tv0, tv0, nullptr, nullptr, nullptr, 0, 0, unused, nullptr, st, nullptr, nullptr);
-            odom_iterate_kernel<true><<<nb_cap, LM_THREADS, 0, c->stream>>>(tv0, tv0, nullptr, nullptr, nullptr, 0, 0, 0, unused,
-                                                                         nullptr, c->partials.p, c->result.p, c->ticket.p,
-                                                                         nullptr, nullptr, st);
-            odom_lm_step_kernel<<<1, 32, 0, c->stream>>>(st, c->result.p, *hp, mbp);
-          });
-      if (rc) return rc;
-      lg.cap_a = cap_sh; lg.cap_b = cap_fl;
-      memcpy(lg.baked, baked, sizeof baked);
-    }
-    LB_CUDA(c, cudaGraphLaunch(lg.exec, c->stream));
-    const int rc = use_mailbox ? lm_wait_mailbox(c, &h) : lm_read_header(c, st, &h);
-    if (rc) return rc;
-    // gate + per executed iteration: search (a no-op except every 5th), iterate, step -- launched by the WHILE node
-    c->launches += 1 + 3 * h.iters_run;
-    g_total_launches.fetch_add(1 + 3 * h.iters_run, std::memory_order_relaxed);
-  } else {
-    for (int it = 0; it < max_iterations;) {
-      const int chunk_end = std::min(max_iterations, it + 5);  // one correspondence search per chunk
-      for (; it < chunk_end; it++) {
-        if (it % 5 == 0) {
-          odom_search_kernel<true><<<blocks_for((long long)(nsh + nfl) * 32, LM_THREADS), LM_THREADS, 0, c->stream>>>(
+  // search + iterate + step per iteration, one correspondence search per chunk of 5
+  const LmLoopShape shape{LM_THREADS, 3, 5, 0, false, LOAM_B200_K_ODOM_ITER};
+  return lm_loop_solve(
+      c, c->odom_loop, &st->h, shape, nsh, nfl, max_iterations,
+      [&](int seq) {
+        odom_lm_init_kernel<<<1, 32, 0, c->stream>>>(st, rot[0], rot[1], rot[2], pos[0], pos[1], pos[2], inv_scan_period,
+                                                     delta_t_abort, delta_r_abort, max_iterations, tc.m, ts.m, io, seq);
+      },
+      [&](int it, int q_sh, int q_fl, int grid) {
+        // (in the graph the search runs every iteration: a no-op except every 5th)
+        const bool search = it % 5 == 0;
+        if (search)
+          odom_search_kernel<true><<<blocks_for((long long)(q_sh + q_fl) * 32, LM_THREADS), LM_THREADS, 0, c->stream>>>(
               tv0, tv0, nullptr, nullptr, nullptr, 0, 0, unused, nullptr, st, nullptr, nullptr);
-          LB_LAUNCH_CHECK(c);
-        }
-        odom_iterate_kernel<true><<<nb, LM_THREADS, 0, c->stream>>>(tv0, tv0, nullptr, nullptr, nullptr, 0, 0, 0, unused, nullptr,
-                                                                  c->partials.p, c->result.p, c->ticket.p, nullptr, nullptr, st);
-        LB_LAUNCH_CHECK(c);
-        odom_lm_step_kernel<<<1, 32, 0, c->stream>>>(st, c->result.p);
-        LB_LAUNCH_CHECK(c);
-      }
-      const int rc = lm_read_header(c, st, &h);
-      if (rc) return rc;
-      if (h.done) break;
-    }
-  }
-  prof_end(c);
-  for (int i = 0; i < 3; i++) { out->rot[i] = h.rot[i]; out->pos[i] = h.pos[i]; }
-  out->iterations = h.iters_run;
-  out->converged = h.done ? 1 : 0;
-  return LOAM_B200_OK;
+        odom_iterate_kernel<true><<<grid, LM_THREADS, 0, c->stream>>>(tv0, tv0, nullptr, nullptr, nullptr, 0, 0, 0, unused,
+                                                                     nullptr, c->partials.p, c->result.p, c->ticket.p,
+                                                                     nullptr, nullptr, st);
+        return search ? 2 : 1;
+      },
+      [&](unsigned long long handle, float* mailbox) {
+        odom_lm_step_kernel<<<1, 32, 0, c->stream>>>(st, c->result.p, handle, mailbox);
+      },
+      out);
 }
 
 int loam_b200_map_solve(loam_b200_ctx* c, const float rot[3], const float pos[3], int max_iterations, float delta_t_abort,
                         float delta_r_abort, loam_b200_lm_result* out) {
   CHECK_CTX(c);
   if (!rot || !pos || !out || max_iterations < 0) return LOAM_B200_ERR_ARG;
-  // a query slice without a communicator only yields partials; the cube-sharded map runs the per-iteration form (its
-  // all-reduce is fused into the iteration kernel)
-  if (c->shard_world > 1 && !c->comm) return LOAM_B200_ERR_STATE;
+  // A query slice without a communicator only yields partials, and the cube-sharded map runs the per-iteration form
+  // (its all-reduce is fused into the iteration kernel).  Past this test shard_slab > 0 implies shard_world == 1, so
+  // map_slice_of's slice is the communicator's query slice of this rank.
+  if (c->shard_world > 1 && (!c->comm || c->shard_slab > 0)) return LOAM_B200_ERR_STATE;
   const int nc = c->map_nc, ns = c->map_ns;
   memset(out, 0, sizeof *out);
   for (int i = 0; i < 3; i++) { out->rot[i] = rot[i]; out->pos[i] = pos[i]; }
   if (nc + ns == 0 || max_iterations == 0) return LOAM_B200_OK;
-  // this rank's contiguous slice of each query kind (everything when not sharded)
-  const int W = c->shard_world, R = c->shard_rank;
-  const int c0 = (int)((long long)nc * R / W), c1 = (int)((long long)nc * (R + 1) / W);
-  const int s0 = (int)((long long)ns * R / W), s1 = (int)((long long)ns * (R + 1) / W);
-  const int lc = c1 - c0, ls = s1 - s0;
-  const int cb = blocks_for(lc, MAP_Q_PER_BLOCK), sb = blocks_for(ls, MAP_Q_PER_BLOCK);
-  const int nb = std::max(cb + sb, 1);
-  const bool use_graph = loop_graphs_enabled() && !c->comm;
-  LoopGraph& lg = c->map_loop;
-  const int cap_c = use_graph ? std::max(lg.cap_a, lc > lg.cap_a ? round_cap(lc) : 0) : lc;
-  const int cap_s = use_graph ? std::max(lg.cap_b, ls > lg.cap_b ? round_cap(ls) : 0) : ls;
-  const int nb_cap = std::max(blocks_for(cap_c, MAP_Q_PER_BLOCK) + blocks_for(cap_s, MAP_Q_PER_BLOCK), 1);
-  LB_CUDA(c, c->partials.reserve((size_t)std::max(nb, nb_cap) * NEQ));
+  const MapSlice q = map_slice_of(c);
   LB_CUDA(c, c->lm_state.reserve(sizeof(OdomLmState) + sizeof(MapLmState)));
   MapLmState* st = reinterpret_cast<MapLmState*>(c->lm_state.p + sizeof(OdomLmState));
-  const bool use_mailbox = use_graph && !c->prof_on && c->result_mailbox.reserve(64) == cudaSuccess;
-  int seq = 0;
-  if (use_mailbox) seq = next_mailbox(c).seq;
   MapLoopIo io;
   memset(&io, 0, sizeof io);
-  if (c->map_use_store) {
-    const MapCellLookup l0 = store_lookup_of(c, 0), l1 = store_lookup_of(c, 1);
-    memcpy(io.lookup[0], &l0, sizeof l0);
-    memcpy(io.lookup[1], &l1, sizeof l1);
-  } else {
-    const GridCellLookup l0{grid_view_of(c->grid[0])}, l1{grid_view_of(c->grid[1])};
-    memcpy(io.lookup[0], &l0, sizeof l0);
-    memcpy(io.lookup[1], &l1, sizeof l1);
-  }
-  io.queries = c->map_q_corner; io.queries_surf = c->map_q_surf; io.n_corner_total = nc; io.c0 = c0; io.n_corner = lc; io.s0 = s0; io.n_surf = ls;
-  io.corner_blocks = cb; io.n_blocks = nb;
-  map_lm_init_kernel<<<1, 128, 0, c->stream>>>(st, rot[0], rot[1], rot[2], pos[0], pos[1], pos[2], delta_t_abort,
-                                               delta_r_abort, max_iterations, io, seq);
-  LB_LAUNCH_CHECK(c);
+  with_map_lookups(c, [&](auto corner, auto surf) {
+    memcpy(io.lookup[0], &corner, sizeof corner);
+    memcpy(io.lookup[1], &surf, sizeof surf);
+  });
+  io.queries = c->map_q_corner; io.queries_surf = c->map_q_surf; io.n_corner_total = nc; io.c0 = q.c0; io.n_corner = q.lc;
+  io.s0 = q.s0; io.n_surf = q.ls; io.corner_blocks = q.cb; io.n_blocks = q.nb;
   const MapIterArgs unused{};
-  LmHeader h{};
-  prof_begin(c, LOAM_B200_K_MAP_ITER);
-  auto launch_iterate = [&](int grid) {
-    if (c->map_use_store)
-      map_iterate_kernel<false, MapCellLookup, true><<<grid, MAP_THREADS, 0, c->stream>>>(
-          MapCellLookup{}, MapCellLookup{}, nullptr, nullptr, 0, 0, 0, 0, 0, 0, unused, c->partials.p, c->result.p, c->ticket.p, nullptr,
-          nullptr, nullptr, st);
-    else
-      map_iterate_kernel<false, GridCellLookup, true><<<grid, MAP_THREADS, 0, c->stream>>>(
-          GridCellLookup{}, GridCellLookup{}, nullptr, nullptr, 0, 0, 0, 0, 0, 0, unused, c->partials.p, c->result.p, c->ticket.p, nullptr,
-          nullptr, nullptr, st);
-  };
-  if (use_graph) {
-    const int variant = c->map_use_store ? 1 : 0;
-    const void* baked[4] = {st, c->partials.p, c->result.p, use_mailbox ? (void*)c->result_mailbox.p : nullptr};
-    if (!lg.exec || lg.cap_a != cap_c || lg.cap_b != cap_s || lg.variant != variant || memcmp(lg.baked, baked, sizeof baked) != 0) {
-      float* mbp = use_mailbox ? c->result_mailbox.p : nullptr;
-      unsigned long long* hp = &lg.handle;
-      const int rc = loop_graph_build(
-          c, lg, [&] { lm_gate_kernel<<<1, 32, 0, c->stream>>>(&st->h, *hp, mbp); },
-          [&] {
-            launch_iterate(nb_cap);
-            map_lm_step_kernel<<<1, 32, 0, c->stream>>>(st, c->result.p, *hp, mbp);
-          });
-      if (rc) return rc;
-      lg.cap_a = cap_c; lg.cap_b = cap_s; lg.variant = variant;
-      memcpy(lg.baked, baked, sizeof baked);
-    }
-    LB_CUDA(c, cudaGraphLaunch(lg.exec, c->stream));
-    const int rc = use_mailbox ? lm_wait_mailbox(c, &h) : lm_read_header(c, st, &h);
-    if (rc) return rc;
-    c->launches += 1 + 2 * h.iters_run;  // gate + (iterate, step) per executed iteration
-    g_total_launches.fetch_add(1 + 2 * h.iters_run, std::memory_order_relaxed);
-  } else {
-    for (int it = 0; it < max_iterations;) {
-      const int chunk_end = std::min(max_iterations, it + 3);  // 2-3 iterations is the usual case
-      for (; it < chunk_end; it++) {
-        launch_iterate(nb);
-        LB_LAUNCH_CHECK(c);
-        {
-          const int rcc = allreduce_result(c);  // no-op without a communicator; every rank then takes the same step
-          if (rcc) return rcc;
-        }
-        map_lm_step_kernel<<<1, 32, 0, c->stream>>>(st, c->result.p);
-        LB_LAUNCH_CHECK(c);
-      }
-      const int rc = lm_read_header(c, st, &h);
-      if (rc) return rc;
-      if (h.done) break;
-    }
-  }
-  prof_end(c);
-  for (int i = 0; i < 3; i++) { out->rot[i] = h.rot[i]; out->pos[i] = h.pos[i]; }
-  out->iterations = h.iters_run;
-  out->converged = h.done ? 1 : 0;
-  return LOAM_B200_OK;
+  // iterate + step per iteration; 2-3 iterations is the usual case
+  const LmLoopShape shape{MAP_Q_PER_BLOCK, 2, 3, c->map_use_store ? 1 : 0, true, LOAM_B200_K_MAP_ITER};
+  return lm_loop_solve(
+      c, c->map_loop, &st->h, shape, q.lc, q.ls, max_iterations,
+      [&](int seq) {
+        map_lm_init_kernel<<<1, 128, 0, c->stream>>>(st, rot[0], rot[1], rot[2], pos[0], pos[1], pos[2], delta_t_abort,
+                                                     delta_r_abort, max_iterations, io, seq);
+      },
+      [&](int, int, int, int grid) {
+        launch_map_iterate<false, true>(c, grid, MapSlice{}, unused, nullptr, nullptr, nullptr, st);
+        return 1;
+      },
+      [&](unsigned long long handle, float* mailbox) {
+        map_lm_step_kernel<<<1, 32, 0, c->stream>>>(st, c->result.p, handle, mailbox);
+      },
+      out);
 }
 
 // The warp-parallel 6 x 6 step of the device-resident loops on caller-supplied normal equations (parity tests: it must

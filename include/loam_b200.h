@@ -620,6 +620,52 @@ int loam_b200_dense_raycast(loam_b200_ctx* ctx, const float* rays, int n, int on
 int loam_b200_debug_dense_ray_index_bytes(loam_b200_ctx* ctx, long long* out);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Distance field of the whole-run voxel map (csrc/densemap.cuh, DESIGN.md "Distance field of the whole-run voxel
+ * map"): how far a point is from the nearest obstacle of the target above, and in which direction that distance grows
+ * -- collision checks, safety margins, trajectory optimisers.  Not on the per-sweep path; the field never feeds back
+ * into the mapping stage.  Unsigned (0 inside obstacles), no unknown space.
+ *   occupied: a voxel whose key is in the target (as for the ray cast: with or without a normal).  L = (double)leaf of
+ *     the target; voxel v spans [v L, (v + 1) L) per axis.
+ *   box: lo[3] (voxel indices, e.g. floorf(c * (1.0f / leaf)) of a corner, api.voxel_box) and dims[3] >= 1, axis-
+ *     aligned in the map frame (the LOAM frame, y up).  Cell (x, y, z) is voxel lo + (x, y, z); x varies fastest,
+ *     then y, then z (numpy shape (nz, ny, nx)).
+ *   value: sq = the squared Euclidean distance in voxel units from the cell's voxel to the nearest occupied voxel of
+ *     the whole target, centre to centre (an integer, 0 on an occupied cell); dist = (float)(sqrt((double)sq) * L).
+ *   range: max_distance (finite, > 0).  A cell is beyond when sqrt((double)sq) * L > (double)max_distance; a beyond
+ *     cell has sq = -1 and dist = +inf.  The exact transform runs over the box grown by pad = floor((double)
+ *     max_distance / L) + 1 voxels on every side: an obstacle within max_distance of a cell lies inside that padded
+ *     box, so every value reported equals the whole-target value and every beyond cell is truly beyond.
+ * build: dist and sq (nx * ny * nz each) may each be NULL (the field is then kept on the device only).  The field (sq,
+ *   4 B per cell) is a snapshot kept with the target: later inserts do not change it, the next build replaces it, a
+ *   target build or load drops it.  The first build after a target build or load also builds the target's ray index
+ *   (loam_b200_dense_raycast) and rasterises from it; an empty target gives a field beyond everywhere and launches
+ *   nothing.  Synchronous.
+ * query: n points (float[4] in the map frame, w ignored; host memory, or device memory when on_device != 0) ->
+ *   dist[n] and, unless grad is NULL, grad[3n] (d dist / d x, y, z per point).  fp64 without FMA, each operation
+ *   rounded on its own, one rounding to float at the end:
+ *     per axis a: g_a = ((double)p_a / L - 0.5) - (double)lo_a; defined when dims_a >= 2 and 0 <= g_a <= dims_a - 1 on
+ *       every axis (a NaN or infinite coordinate never is): then i_a = min((int)floor(g_a), dims_a - 2), f_a = g_a -
+ *       i_a; otherwise dist and grad are NaN.
+ *     corner w(dx, dy, dz) = sqrt((double)sq) * L of cell i + (dx, dy, dz), or (double)max_distance for a beyond
+ *       corner (the query saturates there); lerp(a, b, f) = a + f * (b - a).
+ *     dist = lerp(lerp(lerp(w000, w100, fx), lerp(w010, w110, fx), fy), lerp(lerp(w001, w101, fx), lerp(w011, w111,
+ *       fx), fy), fz)   (w indexed x y z)
+ *     gx = lerp(lerp(w100 - w000, w110 - w010, fy), lerp(w101 - w001, w111 - w011, fy), fz) / L
+ *     gy = lerp(lerp(w010 - w000, w110 - w100, fx), lerp(w011 - w001, w111 - w101, fx), fz) / L
+ *     gz = lerp(lerp(w001 - w000, w101 - w100, fx), lerp(w011 - w010, w111 - w110, fx), fy) / L
+ * No target, or a query without a field: LOAM_B200_ERR_STATE.  LOAM_B200_ERR_ARG for a NULL pointer (lo, dims; xyzi
+ * or dist with n > 0), a non-finite max_distance, unless max_distance > 0, max_distance / leaf <= 1024, every padded
+ * axis dims_a + 2 pad <= 8192, the padded cells <= 2^27 and the padded box inside the key range [-2^20, 2^20).
+ * Launches count under LOAM_B200_K_DENSE.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int loam_b200_dense_distance_build(loam_b200_ctx* ctx, const int lo[3], const int dims[3], float max_distance,
+                                   float* dist, int32_t* sq);
+int loam_b200_dense_distance_query(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device, float* dist,
+                                   float* grad);
+/* Test query: device bytes of the distance field (4 per cell of the box; 0 without a field). */
+int loam_b200_debug_dense_distance_bytes(loam_b200_ctx* ctx, long long* out);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Place recognition and global relocalisation in the whole-run voxel map (csrc/densemap.cuh, DESIGN.md "Place
  * recognition and global relocalisation"): relocalise a cloud with no prior pose -- a robot waking up in a saved map,
  * a tracking loss after a long gap, a second session that starts elsewhere.  A polar height descriptor of the cloud

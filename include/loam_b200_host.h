@@ -145,6 +145,12 @@ int loam_b200_map_dense_relocalize(void* h, const float* xyzi, int n, const floa
  * NULL). */
 int loam_b200_map_dense_raycast(void* h, const float* rays, int n, const float* pose6, float min_range,
                                 float max_range, float* range, int* index);
+/* distance field of that target (BasicLaserMapping::buildDenseDistanceField / queryDenseDistance, include/loam_b200.h
+ * "Distance field of the whole-run voxel map"), same in-flight rule: build over the box lo[3], dims[3] -> dist and sq
+ * (nx * ny * nz each, either may be NULL); query n map-frame points of float[4] -> dist[n], grad[3n] (may be NULL). */
+int loam_b200_map_dense_distance_build(void* h, const int* lo, const int* dims, float max_distance, float* dist,
+                                       int* sq);
+int loam_b200_map_dense_distance_query(void* h, const float* xyzi, int n, float* dist, float* grad);
 /* place recognition and global relocalisation in that target (BasicLaserMapping::buildDensePlaces /
  * queryDensePlaces / relocalizeGlobalInDenseTarget, include/loam_b200.h "Place recognition and global
  * relocalisation"), same in-flight rule: k positions of float[3], n_rays rays and n points of float[4]. */

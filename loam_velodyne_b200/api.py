@@ -230,6 +230,9 @@ def lib():
                                                  C.POINTER(RelocParams), C.POINTER(RelocCandidate), C.c_int, _I]),
         "loam_b200_dense_raycast": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_float, C.c_float, _F, _I]),
         "loam_b200_debug_dense_ray_index_bytes": (C.c_int, [vp, _LL]),
+        "loam_b200_dense_distance_build": (C.c_int, [vp, _I, _I, C.c_float, _F, _I]),
+        "loam_b200_dense_distance_query": (C.c_int, [vp, _F, C.c_int, C.c_int, _F, _F]),
+        "loam_b200_debug_dense_distance_bytes": (C.c_int, [vp, _LL]),
         "loam_b200_place_descriptor": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(PlaceParams), _F]),
         "loam_b200_dense_place_build": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.POINTER(PlaceParams)]),
         "loam_b200_dense_place_query": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_int, C.POINTER(PlaceMatch), _I]),
@@ -300,6 +303,8 @@ def lib():
         "loam_b200_map_dense_relocalize": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.POINTER(RelocParams),
                                                      C.POINTER(RelocCandidate), C.c_int, _I]),
         "loam_b200_map_dense_raycast": (C.c_int, [vp, _F, C.c_int, _F, C.c_float, C.c_float, _F, _I]),
+        "loam_b200_map_dense_distance_build": (C.c_int, [vp, _I, _I, C.c_float, _F, _I]),
+        "loam_b200_map_dense_distance_query": (C.c_int, [vp, _F, C.c_int, _F, _F]),
         "loam_b200_map_dense_place_build": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.POINTER(PlaceParams)]),
         "loam_b200_map_dense_place_query": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(PlaceMatch), _I]),
         "loam_b200_map_dense_relocalize_global": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_float, C.c_int, C.c_float,
@@ -833,6 +838,37 @@ class Ctx:
         self._ck(self.L.loam_b200_debug_dense_ray_index_bytes(self.h, C.byref(out)), "dense_ray_index_bytes")
         return out.value
 
+    # ---- distance field (include/loam_b200.h "Distance field of the whole-run voxel map")
+    def dense_distance_field(self, lo, dims, max_distance, download=True):
+        """Build the distance field of the target over the box of voxels lo + [0, dims) (3 ints each, x y z; see
+        voxel_box) -> (dist float32, sq int32), each shaped (nz, ny, nx): the distance in metres to the nearest target
+        voxel (+inf beyond max_distance) and its square in voxel units (-1 beyond).  download=False keeps the field on
+        the device only and returns (None, None)."""
+        lo_a, dims_a, shape = _box_args(lo, dims)
+        dist = np.zeros(shape, np.float32) if download else None
+        sq = np.zeros(shape, np.int32) if download else None
+        self._ck(self.L.loam_b200_dense_distance_build(self.h, _ip(lo_a), _ip(dims_a), np.float32(max_distance),
+                                                       _fp(dist) if download else None,
+                                                       _ip(sq) if download else None), "dense_distance_field")
+        return dist, sq
+
+    def dense_distance_query(self, pts, on_device=False, n=None, gradient=False):
+        """The last distance field at map-frame pts (N x 4, w ignored), trilinear between cell centres (NaN outside
+        them) -> dist float32[N], or (dist, grad float32[N, 3]) with gradient=True.  With on_device=True, pts is the
+        address of n float[4] in device memory."""
+        ptr, k = _pts_or_device(pts, on_device, n)
+        dist = np.zeros(max(k, 1), np.float32)
+        grad = np.zeros((max(k, 1), 3), np.float32) if gradient else None
+        self._ck(self.L.loam_b200_dense_distance_query(self.h, ptr, k, 1 if on_device else 0, _fp(dist),
+                                                       _fp(grad) if gradient else None), "dense_distance_query")
+        return (dist[:k].copy(), grad[:k].copy()) if gradient else dist[:k].copy()
+
+    def dense_distance_bytes(self):
+        """Test query: device bytes of the distance field (4 per cell of the box; 0 without a field)."""
+        out = C.c_longlong(0)
+        self._ck(self.L.loam_b200_debug_dense_distance_bytes(self.h, C.byref(out)), "dense_distance_bytes")
+        return out.value
+
     # ---- place recognition (include/loam_b200.h "Place recognition and global relocalisation")
     def place_descriptor(self, pts, params=None, on_device=False, n=None):
         """Polar height descriptor of sensor-frame pts (N x 4, w ignored) -> float32 (rings, sectors).  With
@@ -973,6 +1009,14 @@ def _pts_or_device(pts, on_device, n):
         return C.cast(C.c_void_p(int(pts)), _F), int(n)
     a = _pts(pts)
     return _fp(a), a.shape[0]
+
+
+def _box_args(lo, dims):
+    """(lo int32[3], dims int32[3], numpy shape (nz, ny, nx)) of a distance field's box."""
+    lo_a = np.ascontiguousarray(lo, np.int32).reshape(3)
+    dims_a = np.ascontiguousarray(dims, np.int32).reshape(3)
+    shape = tuple(int(d) for d in dims_a[::-1]) if (dims_a >= 1).all() else (0,)
+    return lo_a, dims_a, shape
 
 
 def _place_match(m):
@@ -1243,6 +1287,26 @@ class LaserMapping(_Handle):
                                                     np.float32(max_range), _fp(rng), _ip(idx)), "raycastDenseTarget")
         return rng[:k].copy(), idx[:k].copy()
 
+    def build_dense_distance_field(self, lo, dims, max_distance, download=True):
+        """BasicLaserMapping::buildDenseDistanceField; as Ctx.dense_distance_field."""
+        lo_a, dims_a, shape = _box_args(lo, dims)
+        dist = np.zeros(shape, np.float32) if download else None
+        sq = np.zeros(shape, np.int32) if download else None
+        self._ck(self.L.loam_b200_map_dense_distance_build(self.h, _ip(lo_a), _ip(dims_a), np.float32(max_distance),
+                                                           _fp(dist) if download else None,
+                                                           _ip(sq) if download else None), "buildDenseDistanceField")
+        return dist, sq
+
+    def query_dense_distance(self, pts, gradient=False):
+        """BasicLaserMapping::queryDenseDistance; returns what Ctx.dense_distance_query returns."""
+        a = _pts(pts)
+        k = a.shape[0]
+        dist = np.zeros(max(k, 1), np.float32)
+        grad = np.zeros((max(k, 1), 3), np.float32) if gradient else None
+        self._ck(self.L.loam_b200_map_dense_distance_query(self.h, _fp(a), k, _fp(dist), _fp(grad) if gradient else None),
+                 "queryDenseDistance")
+        return (dist[:k].copy(), grad[:k].copy()) if gradient else dist[:k].copy()
+
     def build_dense_places(self, positions, rays, params=None):
         """BasicLaserMapping::buildDensePlaces; as Ctx.dense_place_build."""
         prm = params if params is not None else PlaceParams.default()
@@ -1502,6 +1566,16 @@ def lidar_rays(elevations_deg, n_az):
     d = np.stack([-np.sin(theta) * np.cos(e), np.broadcast_to(np.sin(e), (e.shape[0], int(n_az))),
                   np.cos(theta) * np.cos(e), np.zeros((e.shape[0], int(n_az)))], axis=-1)
     return np.ascontiguousarray(d.reshape(-1, 4), np.float32)
+
+
+def voxel_box(min_xyz, max_xyz, leaf):
+    """The box of voxels (lo int32[3], dims int32[3]) that covers the map-frame corners min_xyz .. max_xyz (metres,
+    x y z) by the map's voxel rule v = floorf(c * (1.0f / leaf)) in float32: lo = the voxel of min_xyz, dims = the
+    voxel of max_xyz - lo + 1 (at least 1 per axis).  The argument of Ctx.dense_distance_field."""
+    inv = np.float32(1.0) / np.float32(leaf)
+    a = np.floor(np.asarray(min_xyz, np.float32).reshape(3) * inv).astype(np.int64)
+    b = np.floor(np.asarray(max_xyz, np.float32).reshape(3) * inv).astype(np.int64)
+    return a.astype(np.int32), np.maximum(b - a + 1, 1).astype(np.int32)
 
 
 def place_grid(matches, yaw_step_deg=PLACE_YAW_STEP_DEG, yaw_steps=PLACE_YAW_STEPS, xz_step=PLACE_XZ_STEP,

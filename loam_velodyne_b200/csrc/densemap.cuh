@@ -886,6 +886,209 @@ dense_raycast_kernel(const float4* __restrict__ rays, int n, DenseRayArgs a, Den
   index[i] = -1;
 }
 
+// ---- distance field of the target (include/loam_b200.h "Distance field of the whole-run voxel map")
+// Exact squared EDT in voxel units over the padded box (the box grown by pad = floor(max_distance / L) + 1 voxels on
+// every side), separable: x pass (nearest site on each x line, fused with the rasterisation from the ray index), then
+// Meijster's integer lower envelope along y and along z.  Values stay below 3 * 8191^2 < 2^31, so int32 holds every
+// one; DENSE_EDT_INF marks "no site on this line" and never enters a sum.  The y pass only runs the lines whose x lies
+// in the box, and the z pass only those whose x and y do, each writing only the positions inside the box: the rest
+// of the padded box is only ever a source of sites.
+constexpr int DENSE_EDT_INF = 0x7fffffff;
+constexpr int DENSE_EDT_MAX_RATIO = 1024;        // max_distance / leaf
+constexpr int DENSE_EDT_MAX_AXIS = 8192;         // padded cells per axis
+constexpr long long DENSE_EDT_MAX_CELLS = 1ll << 27;  // padded cells
+constexpr int DENSE_EDT_LINE_THREADS = 128;
+
+struct DenseDistArgs {  // by value in the kernel arguments
+  double L, max_distance;
+  int lo[3], n[3];      // the box: first voxel and cells per axis
+};
+
+// x pass, one warp per padded x line (y, z): a lane per cell of each 32-cell chunk probes its brick and tests the bit;
+// a warp max scan carries the nearest site at or left of x forwards, then a min scan the nearest at or right of x
+// backwards.  g = the squared distance to the nearer, DENSE_EDT_INF without a site on the line.  The forward pass
+// leaves the left site's index in g, which the backward pass (same lane, same cell) reads back.
+__global__ void __launch_bounds__(256) dense_edt_x_kernel(DenseBrickIndex ix, int plx, int ply, int plz, int nxp,
+                                                          int nyp, long long lines, int* __restrict__ g) {
+  const long long line = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (line >= lines) return;  // whole warps
+  const int uy = ply + (int)(line % nyp) + DENSE_KEY_BIAS, uz = plz + (int)(line / nyp) + DENSE_KEY_BIAS;
+  int* row = g + line * nxp;
+  int carry = -1;  // the nearest site so far, -1: none
+  for (int x0 = 0; x0 < nxp; x0 += 32) {
+    const int x = x0 + lane;
+    bool occ = false;
+    if (x < nxp) {
+      const int ux = plx + x + DENSE_KEY_BIAS;
+      const long long slot = ix.find(dense_brick(ux, uy, uz));
+      occ = slot >= 0 && ix.test(slot, dense_brick_bit(ux, uy, uz));
+    }
+    int v = occ ? x : -1;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v = max(v, u);
+    }
+    v = max(v, carry);
+    if (x < nxp) row[x] = v;
+    carry = __shfl_sync(0xffffffffu, v, 31);
+  }
+  carry = DENSE_EDT_INF;
+  for (int x0 = (nxp - 1) & ~31; x0 >= 0; x0 -= 32) {
+    const int x = x0 + lane;
+    const int left = x < nxp ? row[x] : -1;
+    int v = left == x ? x : DENSE_EDT_INF;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_down_sync(0xffffffffu, v, o);
+      if (lane + o < 32) v = min(v, u);
+    }
+    v = min(v, carry);
+    if (x < nxp) {
+      const int d = min(left >= 0 ? x - left : DENSE_EDT_INF, v != DENSE_EDT_INF ? v - x : DENSE_EDT_INF);
+      row[x] = d == DENSE_EDT_INF ? DENSE_EDT_INF : d * d;
+    }
+    carry = __shfl_sync(0xffffffffu, v, 0);
+  }
+}
+
+// Meijster's lower envelope of the parabolas (u - s)^2 + f(s) of one line's finite sites, its stacks s, t (the first
+// position where s is the lowest) and f(s) in global scratch at stride `ss` (consecutive threads: consecutive x, so
+// every access is coalesced); the top stays in registers.  Sep is the floor division of (u^2 - s^2 + f(u) - f(s)) by
+// 2 (u - s) in int64.  Ties keep the earlier site (only values are ever read).
+struct DenseEdtEnvelope {
+  int* S;
+  int* T;
+  int* G;
+  long long ss;
+  int q = -1, s = 0, t = 0, gs = 0;  // top of the stacks, q == -1: no site
+
+  __device__ __forceinline__ void load() {
+    s = S[q * ss];
+    t = T[q * ss];
+    gs = G[q * ss];
+  }
+  __device__ __forceinline__ void push(int u, int w, int gu) {
+    q++;
+    s = u;
+    t = w;
+    gs = gu;
+    S[q * ss] = u;
+    T[q * ss] = w;
+    G[q * ss] = gu;
+  }
+  // the envelope of f[0], f[fs], ... f[(m - 1) fs]
+  __device__ __forceinline__ void build(const int* __restrict__ f, long long fs, int m) {
+    for (int u = 0; u < m; u++) {
+      const int gu = f[u * fs];
+      if (gu == DENSE_EDT_INF) continue;
+      while (q >= 0) {
+        const long long a = (long long)(t - s) * (t - s) + gs, b = (long long)(t - u) * (t - u) + gu;
+        if (a <= b) break;
+        if (--q >= 0) load();
+      }
+      if (q < 0) {
+        push(u, 0, gu);
+        continue;
+      }
+      const long long num = ((long long)u * u - (long long)s * s) + ((long long)gu - gs), den = 2ll * (u - s);
+      const long long w = (num >= 0 ? num / den : -((-num + den - 1) / den)) + 1;
+      if (w < m) push(u, (int)w, gu);
+    }
+  }
+  // the lower envelope at u, for u descending from the end of the line (DENSE_EDT_INF without sites)
+  __device__ __forceinline__ int at(int u) {
+    if (q < 0) return DENSE_EDT_INF;
+    while (t > u) {
+      q--;
+      load();
+    }
+    return (u - s) * (u - s) + gs;
+  }
+};
+
+// y pass: one thread per line (x, z) with x in the box and z in the padded box; reads the x pass (padded layout),
+// writes the positions y in the box of b[(z, y, x)] (layout nx x ny x nzp)
+__global__ void __launch_bounds__(DENSE_EDT_LINE_THREADS)
+dense_edt_y_kernel(const int* __restrict__ g, int pad, int nx, int ny, int nxp, int nyp, int nzp, int* __restrict__ b,
+                   int* S, int* T, int* G) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)nx * nzp) return;
+  const int x = (int)(i % nx), z = (int)(i / nx);
+  const long long base = (long long)z * nyp * nx + x;  // the line's stacks: [z][position][x]
+  DenseEdtEnvelope e{S + base, T + base, G + base, nx};
+  e.build(g + (long long)z * nyp * nxp + pad + x, nxp, nyp);
+  int* out = b + (long long)z * ny * nx + x;
+  for (int y = ny - 1; y >= 0; y--) out[(long long)y * nx] = e.at(pad + y);
+}
+
+// z pass: one thread per line (x, y) of the box; reads the y pass, writes the field: sq (-1 beyond) and, with `dist`,
+// the float distance
+__global__ void __launch_bounds__(DENSE_EDT_LINE_THREADS)
+dense_edt_z_kernel(const int* __restrict__ b, int pad, DenseDistArgs a, int nzp, int* S, int* T, int* G,
+                   int* __restrict__ sq, float* __restrict__ dist) {
+  const int nx = a.n[0], ny = a.n[1], nz = a.n[2];
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x, plane = (long long)nx * ny;
+  if (i >= plane) return;
+  DenseEdtEnvelope e{S + i, T + i, G + i, plane};  // stacks: [position][y][x]
+  e.build(b + i, plane, nzp);
+  for (int z = nz - 1; z >= 0; z--) {
+    const int v = e.at(pad + z);
+    const double w = v == DENSE_EDT_INF ? 0.0 : sqrt((double)v) * a.L;
+    const bool beyond = v == DENSE_EDT_INF || w > a.max_distance;
+    sq[z * plane + i] = beyond ? -1 : v;
+    if (dist) dist[z * plane + i] = beyond ? __int_as_float(0x7f800000) : (float)w;
+  }
+}
+
+// Distance query, one thread per point, fp64 without FMA, each operation rounded on its own (the header states the
+// expression order): trilinear in the corner distances along x, then y, then z; the gradient per axis the same lerps
+// of the corner differences along that axis, divided by L.  NaN outside the hull of the cell centres.
+__device__ __forceinline__ double dense_lerp(double a, double b, double f) { return a + f * (b - a); }
+
+__global__ void dense_distance_query_kernel(const float4* __restrict__ p, int n, DenseDistArgs a,
+                                            const int* __restrict__ sq, float* __restrict__ dist,
+                                            float* __restrict__ grad) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const float4 q = p[k];
+  const double c[3] = {(double)q.x, (double)q.y, (double)q.z};
+  int i[3];
+  double f[3];
+  bool ok = true;
+#pragma unroll
+  for (int ax = 0; ax < 3; ax++) {
+    const double g = (c[ax] / a.L - 0.5) - (double)a.lo[ax];
+    ok = ok && a.n[ax] >= 2 && g >= 0.0 && g <= (double)(a.n[ax] - 1);
+    i[ax] = ok ? min((int)floor(g), a.n[ax] - 2) : 0;
+    f[ax] = g - (double)i[ax];
+  }
+  if (!ok) {
+    const float nan = __int_as_float(0x7fffffff);
+    dist[k] = nan;
+    if (grad) grad[3 * k] = grad[3 * k + 1] = grad[3 * k + 2] = nan;
+    return;
+  }
+  const long long sy = a.n[0], sz = (long long)a.n[0] * a.n[1];
+  const long long o = (long long)i[2] * sz + (long long)i[1] * sy + i[0];
+  double w[8];  // w[z * 4 + y * 2 + x]
+#pragma unroll
+  for (int j = 0; j < 8; j++) {
+    const int v = __ldg(&sq[o + ((j >> 2) & 1) * sz + ((j >> 1) & 1) * sy + (j & 1)]);
+    w[j] = v < 0 ? a.max_distance : sqrt((double)v) * a.L;
+  }
+  const double fx = f[0], fy = f[1], fz = f[2];
+  const double x00 = dense_lerp(w[0], w[1], fx), x10 = dense_lerp(w[2], w[3], fx);
+  const double x01 = dense_lerp(w[4], w[5], fx), x11 = dense_lerp(w[6], w[7], fx);
+  dist[k] = (float)dense_lerp(dense_lerp(x00, x10, fy), dense_lerp(x01, x11, fy), fz);
+  if (!grad) return;
+  const double gx = dense_lerp(dense_lerp(w[1] - w[0], w[3] - w[2], fy), dense_lerp(w[5] - w[4], w[7] - w[6], fy), fz);
+  const double gy = dense_lerp(dense_lerp(w[2] - w[0], w[3] - w[1], fx), dense_lerp(w[6] - w[4], w[7] - w[5], fx), fz);
+  const double gz = dense_lerp(dense_lerp(w[4] - w[0], w[5] - w[1], fx), dense_lerp(w[6] - w[2], w[7] - w[3], fx), fy);
+  grad[3 * k] = (float)(gx / a.L);
+  grad[3 * k + 1] = (float)(gy / a.L);
+  grad[3 * k + 2] = (float)(gz / a.L);
+}
+
 // ---- place descriptors and global relocalisation (include/loam_b200.h "Place recognition")
 // Polar height descriptor, rings x sectors cells (ring-major), each the float bits of the largest value v > 0 of its
 // points (0: none).  Bits of non-negative floats order like the floats, so atomicMax gives the same cell in any order.
@@ -1272,6 +1475,14 @@ struct DenseTarget {
   DevBuf<double2> place_tab;            // sector boundaries of the call's params
   DevBuf<double> place_dist;            // per candidate: best distance and shift of the last query
   DevBuf<int> place_shift;
+  // distance field of loam_b200_dense_distance_build: the box's sq field (dist_ready false: none; a build, load or
+  // release drops it), the EDT's scratch (kept for the next build) and the query's outputs
+  bool dist_ready = false;
+  DenseDistArgs dist_args{};
+  DevBuf<int> dist_sq;
+  DevBuf<float> dist_f;                 // the float distances of a build that downloads them
+  DevBuf<int> edt_g, edt_b, edt_s, edt_t, edt_v;
+  DevBuf<float> qdist, qgrad;
 
   void release() {
     keys.release(); keys64.release(); cent.release(); nrm.release(); pts.release(); args.release(); partials.release();
@@ -1282,6 +1493,9 @@ struct DenseTarget {
     place_shift.release();
     place_pos.clear();
     place_k = 0;
+    dist_sq.release(); dist_f.release(); edt_g.release(); edt_b.release(); edt_s.release(); edt_t.release();
+    edt_v.release(); qdist.release(); qgrad.release();
+    dist_ready = false;
     ray = DenseBrickIndex{};
     n = 0;
     ready = false;

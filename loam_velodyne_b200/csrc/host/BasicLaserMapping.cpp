@@ -299,6 +299,28 @@ void BasicLaserMapping::raycastDenseTarget(const Cloud& rays, const Twist& pose,
   if (index) index->assign(idx.begin(), idx.end());
 }
 
+void BasicLaserMapping::buildDenseDistanceField(const int lo[3], const int dims[3], float maxDistance,
+                                                std::vector<float>* dist, std::vector<int>* sq) {
+  size_t n = 0;
+  if (lo && dims && dims[0] > 0 && dims[1] > 0 && dims[2] > 0) n = (size_t)dims[0] * dims[1] * dims[2];
+  std::vector<int32_t> s(sq ? n : 0);
+  if (dist) dist->resize(n);
+  _gpu->check(loam_b200_dense_distance_build(_gpu->get(), lo, dims, maxDistance, dist ? dist->data() : nullptr,
+                                             sq ? s.data() : nullptr),
+              "loam_b200_dense_distance_build");
+  if (sq) sq->assign(s.begin(), s.end());
+}
+
+void BasicLaserMapping::queryDenseDistance(const Cloud& points, std::vector<float>& dist, std::vector<float>* grad) {
+  b200::pack(points, _bufA);
+  const size_t n = points.points.size();
+  dist.resize(n);
+  if (grad) grad->resize(3 * n);
+  _gpu->check(loam_b200_dense_distance_query(_gpu->get(), _bufA.data(), (int)n, 0, dist.data(),
+                                             grad ? grad->data() : nullptr),
+              "loam_b200_dense_distance_query");
+}
+
 static loam_b200_place_params placeParamsOf(const BasicLaserMapping::PlaceParams& p) {
   return loam_b200_place_params{p.rings, p.sectors, p.maxRadius, p.heightOffset, p.minRange, p.maxRange};
 }

@@ -710,6 +710,39 @@ int loam_b200_map_dense_raycast(void* h, const float* rays, int n, const float* 
     return 0;
   });
 }
+int loam_b200_map_dense_distance_build(void* h, const int* lo, const int* dims, float max_distance, float* dist,
+                                       int* sq) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (!lo || !dims) {
+    g_err = "loam_b200_map_dense_distance_build: NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    std::vector<float> d;
+    std::vector<int> s;
+    m->m.buildDenseDistanceField(lo, dims, max_distance, dist ? &d : nullptr, sq ? &s : nullptr);
+    if (dist) std::memcpy(dist, d.data(), d.size() * sizeof(float));
+    if (sq) std::memcpy(sq, s.data(), s.size() * sizeof(int));
+    return 0;
+  });
+}
+int loam_b200_map_dense_distance_query(void* h, const float* xyzi, int n, float* dist, float* grad) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && (!xyzi || !dist))) {
+    g_err = "loam_b200_map_dense_distance_query: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, xyzi, n);
+    std::vector<float> d, g;
+    m->m.queryDenseDistance(m->scratchA, d, grad ? &g : nullptr);
+    if (n > 0) std::memcpy(dist, d.data(), (size_t)n * sizeof(float));
+    if (grad && n > 0) std::memcpy(grad, g.data(), (size_t)3 * n * sizeof(float));
+    return 0;
+  });
+}
 static loam::BasicLaserMapping::PlaceParams place_params_of(const loam_b200_place_params& p) {
   loam::BasicLaserMapping::PlaceParams o;
   o.rings = p.rings;

@@ -213,6 +213,15 @@ class BasicLaserMapping {
   // none; index (optional) its position in the target, -1 when none.
   void raycastDenseTarget(const pcl::PointCloud<pcl::PointXYZI>& rays, const Twist& pose, float minRange,
                           float maxRange, std::vector<float>& range, std::vector<int>* index = nullptr);
+  // Distance field of the target (include/loam_b200.h "Distance field of the whole-run voxel map"): exact distances to
+  // the nearest target voxel in the box of voxels lo + [0, dims), kept on the device.  dist / sq (optional) receive
+  // the box's float distances (+inf beyond maxDistance) and squared voxel distances (-1 beyond), x fastest.
+  // queryDenseDistance interpolates the field at map-frame points: dist per point (NaN outside the box's cell
+  // centres) and, optionally, its gradient (3 floats per point).
+  void buildDenseDistanceField(const int lo[3], const int dims[3], float maxDistance, std::vector<float>* dist = nullptr,
+                               std::vector<int>* sq = nullptr);
+  void queryDenseDistance(const pcl::PointCloud<pcl::PointXYZI>& points, std::vector<float>& dist,
+                          std::vector<float>* grad = nullptr);
   // Place recognition and global relocalisation (include/loam_b200.h "Place recognition and global relocalisation"),
   // for a cloud with no prior pose.  buildDensePlaces renders a polar height descriptor at each position from the
   // target through the ray cast (rays: a sensor's directions); the database lives with the target.  queryDensePlaces

@@ -222,6 +222,15 @@ int loam_b200_map_solve(loam_b200_ctx* ctx, const float rot[3], const float pos[
 int loam_b200_debug_gn_solve(loam_b200_ctx* ctx, const float* ata_atb, int n, int first_iteration, float eigen_threshold,
                              float* x_out, int* degenerate_out);
 
+/* Test hook: the radix sort every stage shares (8 bits per pass, min(ceil(key_bits / 8), 4) passes) on n host pairs.
+ * n_live >= 0 is passed as the sort's device-side live count (only the first min(n, n_live) pairs are sorted and
+ * returned meaningfully); n_live < 0 passes none.  out_params == 0 sorts as the callers that read the first buffer
+ * directly (an even number of passes).  keys_out / vals_out receive n entries; *path_out the path that ran: 0 the
+ * one-cluster sort (0 < n <= 131072 and clusters usable), 1 onesweep with 4 items per thread (n < 200000), 2 onesweep
+ * with 16, -1 nothing (n == 0).  LOAM_B200_ERR_ARG for a NULL pointer, n < 0 or key_bits outside 1..32. */
+int loam_b200_debug_sort_pairs(loam_b200_ctx* ctx, const uint32_t* keys, const int32_t* vals, int n, int n_live,
+                               int key_bits, int out_params, uint32_t* keys_out, int32_t* vals_out, int* path_out);
+
 /* BasicLaserOdometry::transformToEnd (BasicLaserOdometry.cpp:57-87) without IMU terms, in place on n host points */
 int loam_b200_transform_to_end(loam_b200_ctx* ctx, float* pts, int n, const loam_b200_odom_pose* pose);
 /* pointAssociateToMap over n host points in place (BasicLaserMapping.cpp:207-219, 235-240) */

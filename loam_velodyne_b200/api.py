@@ -173,6 +173,7 @@ def lib():
         "loam_b200_odom_iterate": (C.c_int, [vp, C.POINTER(OdomPose), C.POINTER(NormalEq)]),
         "loam_b200_odom_iterate_debug": (C.c_int, [vp, C.POINTER(OdomPose), C.POINTER(NormalEq), _F, _B, _I]),
         "loam_b200_debug_gn_solve": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_float, _F, _I]),
+        "loam_b200_debug_sort_pairs": (C.c_int, [vp, _U, _I, C.c_int, C.c_int, C.c_int, C.c_int, _U, _I, _I]),
         "loam_b200_transform_to_end": (C.c_int, [vp, _F, C.c_int, C.POINTER(OdomPose)]),
         "loam_b200_transform_to_map": (C.c_int, [vp, _F, C.c_int, C.POINTER(Pose)]),
         "loam_b200_voxel_grid": (C.c_int, [vp, _F, C.c_int, C.c_float, _F, C.c_int, _I]),
@@ -620,6 +621,25 @@ class Ctx:
         self._ck(self.L.loam_b200_debug_gn_solve(self.h, _fp(packed), n, 1 if first_iteration else 0, eigen_threshold,
                                                  _fp(x), _ip(deg)), "debug_gn_solve")
         return x, deg
+
+    def debug_sort_pairs(self, keys, vals, key_bits, live=None, out_params=True):
+        """The shared radix sort on (keys uint32, vals int32) -> (keys, vals, path): only the first min(n, live) entries
+        are sorted (live=None: all); path 0 one-cluster sort, 1 onesweep with 4 items per thread, 2 with 16, -1 none."""
+        k = np.ascontiguousarray(keys, dtype=np.uint32).reshape(-1)
+        v = np.ascontiguousarray(vals, dtype=np.int32).reshape(-1)
+        if k.shape != v.shape:
+            raise ValueError("keys and vals differ in length")
+        n = k.shape[0]
+        ko = np.zeros(max(n, 1), np.uint32)
+        vo = np.zeros(max(n, 1), np.int32)
+        path = C.c_int(-1)
+        kin = k if n else np.zeros(1, np.uint32)  # never a NULL pointer
+        vin = v if n else np.zeros(1, np.int32)
+        self._ck(self.L.loam_b200_debug_sort_pairs(self.h, kin.ctypes.data_as(_U), _ip(vin), n,
+                                                   -1 if live is None else int(live), int(key_bits),
+                                                   1 if out_params else 0, ko.ctypes.data_as(_U), _ip(vo),
+                                                   C.byref(path)), "debug_sort_pairs")
+        return ko[:n].copy(), vo[:n].copy(), path.value
 
     def odom_solve(self, twist6, scan_period=0.1, max_iter=25, delta_t=0.1, delta_r=0.1):
         """Whole scan-to-scan Gauss-Newton loop on the device -> (twist6, iterations)."""

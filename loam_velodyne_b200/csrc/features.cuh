@@ -327,7 +327,8 @@ feature_ring_kernel(const float4* __restrict__ pts, const int* __restrict__ ring
       const int i0 = (int)(floorf(p.x * inv) - (float)minb0);
       const int i1 = (int)(floorf(p.y * inv) - (float)minb1);
       const int i2 = (int)(floorf(p.z * inv) - (float)minb2);
-      const unsigned vidx = (unsigned)(i0 + i1 * div0 + i2 * div0 * div1);
+      // unsigned: pcl's int32 key wraps (defined behaviour here) when the div product passes 2^31
+      const unsigned vidx = (unsigned)i0 + (unsigned)i1 * (unsigned)div0 + (unsigned)i2 * (unsigned)div0 * (unsigned)div1;
       key = ((unsigned long long)vidx << 32) | (unsigned)t;
     }
     vkeys[t] = key;

@@ -1475,6 +1475,38 @@ int loam_b200_debug_gn_solve(loam_b200_ctx* c, const float* ata_atb, int n, int 
   return LOAM_B200_OK;
 }
 
+int loam_b200_debug_sort_pairs(loam_b200_ctx* c, const uint32_t* keys, const int32_t* vals, int n, int n_live,
+                               int key_bits, int out_params, uint32_t* keys_out, int32_t* vals_out, int* path_out) {
+  CHECK_CTX(c);
+  if (!keys || !vals || !keys_out || !vals_out || !path_out || n < 0 || key_bits < 1 || key_bits > 32)
+    return LOAM_B200_ERR_ARG;
+  // the choice radix_sort_pairs makes
+  *path_out = cluster_path_ok(c, n) ? 0 : n <= 0 ? -1 : rs_items_for(n) == 4 ? 1 : 2;
+  if (n == 0) return LOAM_B200_OK;
+  SortScratch& s = c->sort;
+  LB_CUDA(c, s.keys_a.reserve(n));
+  LB_CUDA(c, s.keys_b.reserve(n));
+  LB_CUDA(c, s.vals_a.reserve(n));
+  LB_CUDA(c, s.vals_b.reserve(n));
+  LB_CUDA(c, cudaMemcpyAsync(s.keys_a.p, keys, (size_t)n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+  LB_CUDA(c, cudaMemcpyAsync(s.vals_a.p, vals, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  const int* n_dev = nullptr;
+  if (n_live >= 0) {  // the live count in device memory, as a compaction earlier on the stream leaves it
+    LB_CUDA(c, c->vox_key.reserve(1));
+    LB_CUDA(c, cudaMemcpyAsync(c->vox_key.p, &n_live, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    n_dev = reinterpret_cast<const int*>(c->vox_key.p);
+  }
+  unsigned* ko = s.keys_a.p;  // callers without out-params read buffer a
+  int* vo = s.vals_a.p;
+  const int rc = out_params ? radix_sort_pairs(c, n, key_bits, &ko, &vo, n_dev)
+                            : radix_sort_pairs(c, n, key_bits, nullptr, nullptr, n_dev);
+  if (rc) return rc;
+  LB_CUDA(c, cudaMemcpyAsync(keys_out, ko, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+  LB_CUDA(c, cudaMemcpyAsync(vals_out, vo, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  LB_CUDA(c, cudaStreamSynchronize(c->stream));
+  return LOAM_B200_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ bulk transforms
 int loam_b200_transform_to_end(loam_b200_ctx* c, float* pts, int n, const loam_b200_odom_pose* p) {
   CHECK_CTX(c);

@@ -83,13 +83,14 @@ __device__ __forceinline__ VoxMeta voxel_meta_from_bbox(const float* mn, const f
 }
 
 // on overflow every point keeps its own key (= its index), which makes the filter an identity exactly like pcl's
-// early return
+// early return.  The guard bounds the truncated extents, not the div product, so keys can pass 2^31: pcl's int32 key
+// wraps there, which is computed in unsigned arithmetic (same bits, no signed overflow).
 __device__ __forceinline__ unsigned voxel_key_of(const float4& q, float inv, const VoxMeta& m, int i) {
   if (m.overflow) return (unsigned)i;
   const int i0 = (int)(floorf(q.x * inv) - (float)m.minb0);
   const int i1 = (int)(floorf(q.y * inv) - (float)m.minb1);
   const int i2 = (int)(floorf(q.z * inv) - (float)m.minb2);
-  return (unsigned)(i0 + i1 * m.div0 + i2 * m.div0 * m.div1);
+  return (unsigned)i0 + (unsigned)i1 * (unsigned)m.div0 + (unsigned)i2 * (unsigned)m.div0 * (unsigned)m.div1;
 }
 
 __global__ void voxel_meta_kernel(const unsigned* __restrict__ bb, float inv, VoxMeta* __restrict__ meta) {

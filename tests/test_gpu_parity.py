@@ -37,14 +37,34 @@ def _features_equal(ctx, chk, pts, rs, **cfg):
     return f
 
 
-@pytest.mark.parametrize("lidar_name", ["vlp16", "hdl64", "dense128"])
+def _lidar(name):
+    """A sensor of synth.Lidar by name; "vlp16_<n>" is VLP-16 geometry with n points per ring."""
+    from loam_velodyne_b200 import synth
+    if name.startswith("vlp16_"):
+        return synth.Lidar.vlp16(int(name.split("_")[1]))
+    return getattr(synth.Lidar, name)()
+
+
+# 4097 and 5344 points per ring: the first ring size that sorts 8192 keys in shared memory, and the largest that fits
+@pytest.mark.parametrize("lidar_name", ["vlp16", "hdl64", "dense128", "vlp16_4097", "vlp16_5344"])
 def test_features_bit_exact(ctx, checker, scene, lidar_name):
     from loam_velodyne_b200 import synth
-    lidar = getattr(synth.Lidar, lidar_name)()
+    lidar = _lidar(lidar_name)
     for sweep in (0, 7):
         pts, rs = synth.make_sweep(scene, lidar, sweep, yaw_rate=math.radians(5.0))
+        if lidar_name.startswith("vlp16_"):
+            assert rs.max() == lidar.n_az
         f = _features_equal(ctx, checker, pts, rs)
         assert len(f["sharp"]) <= lidar.n_rings * 12 and len(f["flat"]) <= lidar.n_rings * 24
+
+
+def test_features_ring_too_long(ctx, scene):
+    """A ring of 5345 points needs more than the 200 KB of shared memory the feature kernel may use."""
+    from loam_velodyne_b200 import api, synth
+    pts, rs = synth.make_sweep(scene, _lidar("vlp16_5345"), 0, yaw_rate=math.radians(5.0))
+    assert rs.max() == 5345
+    with pytest.raises(api.LoamB200Error, match="output capacity too small"):
+        ctx.extract_features(pts, rs)
 
 
 def test_features_ragged_and_empty_rings(ctx, checker, scene):
@@ -316,12 +336,25 @@ def test_ring_binning_front_end(ctx, checker, scene):
     oracle: ring sizes and point order bit-exact, xyz bit-exact, intensity (ring + relTime) within one float ulp at 64
     (the azimuth goes through a double atan2 rounded once instead of the host's float libm)."""
     from loam_velodyne_b200 import api, synth
-    for lidar, bounds, jitter in ((synth.Lidar.vlp16(), (-15.0, 15.0, 16), 0.0), (synth.Lidar.hdl64(), (-24.9, 2.0, 64), 0.15)):
+    old = os.environ.get("LOAM_B200_NO_CLUSTER")
+    os.environ["LOAM_B200_NO_CLUSTER"] = "1"
+    try:
+        nc_ctx = api.Ctx(0)  # the ring sort on onesweep at 4 items instead of one cluster
+    finally:
+        if old is None:
+            del os.environ["LOAM_B200_NO_CLUSTER"]
+        else:
+            os.environ["LOAM_B200_NO_CLUSTER"] = old
+    # dense128: 524 288 + 37 points, the one-pass ring sort on onesweep at 16 items
+    for c, lidar, bounds, jitter in ((ctx, synth.Lidar.vlp16(), (-15.0, 15.0, 16), 0.0),
+                                     (nc_ctx, synth.Lidar.vlp16(), (-15.0, 15.0, 16), 0.0),
+                                     (ctx, synth.Lidar.hdl64(), (-24.9, 2.0, 64), 0.15),
+                                     (ctx, synth.Lidar.dense128(), (-25.0, 15.0, 128), 0.0)):
         pts, rs = synth.make_sweep(scene, lidar, 2, yaw_rate=math.radians(5.0))
         raw = synth.raw_cloud_from_sweep(pts, rs, n_bad=37, seed=5, elev_jitter_deg=jitter)
         ref = checker.multiscan(*bounds)
         p_ref, s_ref = ref.process(raw)
-        p_gpu, s_gpu = ctx.reg_bin(raw, *bounds)
+        p_gpu, s_gpu = c.reg_bin(raw, *bounds)
         np.testing.assert_array_equal(s_gpu, s_ref)
         np.testing.assert_array_equal(p_gpu[:, :3], p_ref[:, :3])
         np.testing.assert_allclose(p_gpu[:, 3], p_ref[:, 3], rtol=0, atol=8e-6)
@@ -333,6 +366,7 @@ def test_ring_binning_front_end(ctx, checker, scene):
             assert g.shape == r.shape
             np.testing.assert_array_equal(g[:, :3], r[:, :3])
             np.testing.assert_allclose(g[:, 3], r[:, 3], rtol=0, atol=8e-6)
+    nc_ctx.close()
     # empty and all-rejected inputs
     p0, s0 = ctx.reg_bin(np.zeros((0, 3), np.float32), -15.0, 15.0, 16)
     assert p0.shape[0] == 0 and s0.sum() == 0

@@ -126,9 +126,10 @@ struct GaussNewtonSolver {
   void solve(const loam_b200_normal_eq& ne, bool firstIteration, float eigenThreshold, float x[6]);
 };
 
-// The Gauss-Newton loops run through loam_b200_odom_solve / loam_b200_map_solve: pose kept on the device, the whole loop
-// one launch of a CUDA graph with a WHILE node (csrc/lmstep.cuh, loam_b200.cu), one host round trip per loop.
-// LOAM_B200_DEVICE_LOOP=0 selects the round-1 form (one kernel + host solve per iteration).
+// LOAM_B200_DEVICE_LOOP=1 (read once per process) runs the Gauss-Newton loops through loam_b200_odom_solve /
+// loam_b200_map_solve: pose kept on the device, the whole loop one launch of a CUDA graph with a WHILE node
+// (csrc/lmstep.cuh, loam_b200.cu), one host round trip per loop.  Unset or any other value: one iteration kernel and
+// one host solve per iteration (the default).
 bool deviceResidentLoops();
 
 // host-side pcl::VoxelGrid replacement: one GPU call

@@ -18,6 +18,6 @@ if len(sys.argv) > 1:
         print(sys.argv[1], i, "it", pg.odom.last_iterations(), pg.mapping.last_iterations(), "od", np.abs(od_g - od_c).max(), "aft", np.abs(aft_g - aft_c).max())
         print("   od_g", od_g, "\n   od_c", od_c, "\n   aft_g", aft_g, "\n   aft_c", aft_c)
 else:
-    for name, env in (("hostloop", {"LOAM_B200_DEVICE_LOOP": "0"}), ("graph", {})):
+    for name, env in (("hostloop", {"LOAM_B200_DEVICE_LOOP": "0"}), ("graph", {"LOAM_B200_DEVICE_LOOP": "1"})):
         e = dict(os.environ); e.update(env)
         subprocess.run([sys.executable, __file__, name], env=e)

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """What carve mode of the whole-run voxel map's visibility pass costs, beside the range-image mode.
 
-Workload: BASELINE config 3 (HDL-64E 64 x 2048 sweeps against a 1 M-point surrounding map), the whole-run map at
---leaf in every arm.  The streaming throughput is timed for the map only, the range-image mode (1 deg x 2 deg, 1 m)
-and carve mode (--margin, --max-range), in alternating windows of --steps sweeps on a fresh pipeline each (after
---warmup sweeps), repeated until each arm has --min-seconds of timed windows (at least three).  Kernel times come from
-a replay of the stream's registered clouds and poses into a kernel-level context, with CUDA-event profiling (family
-"dense") switched on around one call at a time:
+Workload: hdl64_1m streaming (tools/dense_cost.py), the whole-run map at --leaf in every arm.  The streaming
+throughput is timed for the map only, the range-image mode (1 deg x 2 deg, 1 m) and carve mode (--margin,
+--max-range), in alternating windows of --steps sweeps on a fresh pipeline each (after --warmup sweeps), repeated until
+each arm has --min-seconds of timed windows (at least three).  Kernel times come from a replay of the stream's
+registered clouds and poses into a kernel-level context, with CUDA-event profiling (family "dense") switched on around
+one call at a time:
   * the carve pass per sweep at max_range 50 m and 100 m, and the insertion with carve mode off and on (the difference
     is the index's incremental update);
   * both modes' passes at two map sizes: the run's own map, then the same sweeps replayed --replicas more times,
@@ -19,35 +19,14 @@ from __future__ import annotations
 
 import argparse
 import json
-import math
-import os
 import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
 sys.dont_write_bytecode = True
+from dense_cost import gpu_info, hdl64_1m, require_cuda, stats, stream_windows  # noqa: E402
 
 H_RES, V_RES, VIS_MARGIN = 1.0, 2.0, 1.0
-
-
-def gpu_info():
-    try:
-        import pynvml
-        pynvml.nvmlInit()
-        h = pynvml.nvmlDeviceGetHandleByIndex(0)
-        name = pynvml.nvmlDeviceGetName(h)
-        return {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": round(pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0, 1)}
-    except Exception:
-        import torch
-        return {"name": torch.cuda.get_device_name(0), "power_limit_w": None}
-
-
-def med(xs):
-    return round(float(np.median(xs)), 4)
 
 
 def main():
@@ -62,22 +41,14 @@ def main():
     ap.add_argument("--max-windows", type=int, default=20)
     args = ap.parse_args()
 
-    import torch
-    from loam_velodyne_b200 import api, synth
-    if not torch.cuda.is_available():
-        raise SystemExit("dense_carve_cost: no CUDA device (nothing here runs on the CPU)")
-    scene = synth.make_scene()
-    lidar = synth.Lidar.hdl64()
-    corner, surf = synth.make_map(scene, 1_000_000)
-    n = args.warmup + args.steps
-    sweeps = [synth.make_sweep(scene, lidar, i, yaw_rate=math.radians(5.0)) for i in range(n)]
-    d_sweeps = [torch.from_numpy(p).to("cuda:0") for p, _ in sweeps]
-    torch.cuda.synchronize()
+    require_cuda("dense_carve_cost")
+    from loam_velodyne_b200 import api
+    _, _, seed, sweeps = hdl64_1m(args.warmup + args.steps)
     arms = ("map_only", "range_image", "carve")
 
     def pipeline(arm):
         p = api.Pipeline()
-        p.seed_map(corner, surf)
+        p.seed_map(*seed)
         p.mapping.enable_dense_map(args.leaf)
         if arm == "range_image":
             p.mapping.enable_dense_visibility(H_RES, V_RES, VIS_MARGIN)
@@ -85,44 +56,8 @@ def main():
             p.mapping.enable_dense_carving(args.margin, args.max_range)
         return p
 
-    def window(arm):
-        p = pipeline(arm)
-
-        def run(lo, hi):
-            got = 0
-            for i in range(lo, hi):
-                p.submit(ring_sizes=sweeps[i][1], device_ptr=d_sweeps[i].data_ptr())
-                if p.collect(wait=False) is not None:
-                    got += 1
-            while got < hi - lo:
-                p.collect(wait=True)
-                got += 1
-            p.sync()
-
-        run(0, args.warmup)
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        run(args.warmup, n)
-        torch.cuda.synchronize()
-        el = time.perf_counter() - t0
-        del p
-        return el
-
-    windows = {a: [] for a in arms}
-    while True:
-        for a in arms:
-            windows[a].append(window(a))
-        if all(sum(windows[a]) >= args.min_seconds and len(windows[a]) >= 3 for a in arms) or \
-                len(windows["carve"]) >= args.max_windows:
-            break
-
-    def rate(els):
-        s = sorted(els)
-        sps = [args.steps / e for e in s]
-        return {"sweeps_per_s_median": round(args.steps / s[len(s) // 2], 1), "sweeps_per_s_min": round(min(sps), 1),
-                "sweeps_per_s_max": round(max(sps), 1), "windows": len(s)}
-
-    streaming = {a: rate(windows[a]) for a in arms}
+    rates, _ = stream_windows(args, sweeps, pipeline, arms)
+    streaming = {a: {k: v for k, v in r.items() if k != "window_ms_min_median_max"} for a, r in rates.items()}
 
     # the registered clouds and optimised poses of the stream (the pass never changes them)
     seq = pipeline("map_only")
@@ -192,8 +127,8 @@ def main():
             c.cloud_upload(api.C_MAP_FULL, f)
             cv.append(timed(c, lambda: c.dense_observe(api.C_MAP_FULL, pose))[0])
         c.dense_carving(0.0, 0.0)
-        res["range_image_gpu_ms_median"] = med(ri)
-        res["carve_gpu_ms_median"] = med(cv)
+        res["range_image_gpu_ms_median"] = stats(ri)["median"]
+        res["carve_gpu_ms_median"] = stats(cv)["median"]
         res["voxels"] = c.dense_stats()["voxels"]
         res["table_slots"] = c.dense_table_slots()
         return res
@@ -204,6 +139,7 @@ def main():
         insert_all(500.0 * k)
     scaling.append(both_passes())
     c.close()
+    insert_ms = {k: stats([m for m, _ in main_r[f"insert_{k}"]])["median"] for k in ("off", "on")}
 
     out = {
         "workload": "hdl64_1m streaming (BASELINE config 3), inputs in HBM, whole-run map on in every arm",
@@ -215,12 +151,11 @@ def main():
                                                        streaming["map_only"]["sweeps_per_s_median"] - 1.0), 2),
         "range_image_change_vs_map_only_pct": round(100.0 * (streaming["range_image"]["sweeps_per_s_median"] /
                                                              streaming["map_only"]["sweeps_per_s_median"] - 1.0), 2),
-        "carve_gpu_ms_per_sweep_median": {f"{mr:g}m": med([m for m, _ in r["observe"]]) for mr, r in per_range.items()},
+        "carve_gpu_ms_per_sweep_median": {f"{mr:g}m": stats([m for m, _ in r["observe"]])["median"]
+                                          for mr, r in per_range.items()},
         "carve_launches_per_sweep": main_r["observe"][-1][1],
-        "insert_gpu_ms_median": {"carve_off": med([m for m, _ in main_r["insert_off"]]),
-                                 "carve_on": med([m for m, _ in main_r["insert_on"]])},
-        "index_update_gpu_ms_per_sweep": round(med([m for m, _ in main_r["insert_on"]]) -
-                                               med([m for m, _ in main_r["insert_off"]]), 4),
+        "insert_gpu_ms_median": {"carve_off": insert_ms["off"], "carve_on": insert_ms["on"]},
+        "index_update_gpu_ms_per_sweep": round(insert_ms["on"] - insert_ms["off"], 4),
         "insert_launches": {"carve_off": main_r["insert_off"][-1][1], "carve_on": main_r["insert_on"][-1][1]},
         "points_per_sweep": int(np.mean([f.shape[0] for f in fulls])),
         "voxels_after_run": main_r["voxels"], "index_bricks": main_r["bricks"],

@@ -1,10 +1,8 @@
 #!/usr/bin/env python
 """What the distance field of the whole-run voxel map costs.
 
-Workload: the map of tools/dense_raycast_cost.py -- BASELINE config 3 (HDL-64E 64 x 2048 sweeps against a 1 M-point
-surrounding map), --sweeps sweeps through the pipeline, their registered clouds replayed into a kernel-level context
-with the whole-run map at --leaf, and the target built from it (radius 2).  Reported, with the card's name and power
-limit read in the same run:
+Workload: the replayed hdl64_1m map (tools/dense_cost.py), --sweeps sweeps at --leaf, and the target built from it
+(radius 2).  Reported, with the card's name and power limit read in the same run:
   * field builds (kept on the device, no download) of a 40 x 40 x 8 m and a 100 x 100 x 12 m box centred on the last
     mapped pose at max_distance 2 m and 5 m, alternating round by round, --reps rounds after one warm-up: GPU time
     (CUDA-event profiling, family "dense"), median, min and max; cells/s of the box; the algorithmic bytes (the
@@ -21,22 +19,14 @@ from __future__ import annotations
 import argparse
 import json
 import math
-import os
 import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.dont_write_bytecode = True
+from dense_cost import dense_ctx, gpu_info, profiled, replay_run, require_cuda, stats  # noqa: E402
 
 HBM_TBPS = 3.35  # H100 SXM HBM3 peak
-
-
-def stats(v):
-    return {"median": round(float(np.median(v)), 4), "min": round(float(np.min(v)), 4),
-            "max": round(float(np.max(v)), 4)}
 
 
 def algorithmic_bytes(dims, pad):
@@ -55,30 +45,11 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     args = ap.parse_args()
 
+    require_cuda("dense_distance_cost")
     import torch
-    from dense_raycast_cost import gpu_info
-    from loam_velodyne_b200 import api, synth
-    if not torch.cuda.is_available():
-        raise SystemExit("dense_distance_cost: no CUDA device (nothing here runs on the CPU)")
-    scene = synth.make_scene()
-    lidar = synth.Lidar.hdl64()
-    corner, surf = synth.make_map(scene, 1_000_000)
-    seq = api.Pipeline()
-    seq.seed_map(corner, surf)
-    fulls, twists = [], []
-    for i in range(args.sweeps):
-        seq.sweep(*synth.make_sweep(scene, lidar, i, yaw_rate=math.radians(5.0)))
-        fulls.append(seq.mapping.cloud("full"))
-        twists.append(seq.mapping.twist("aft"))
-    seq.sync()
-    del seq
-
-    c = api.Ctx(0)
-    c.dense_enable(args.leaf)
-    for f in fulls:
-        c.cloud_upload(api.C_MAP_FULL, f)
-        c.dense_insert(api.C_MAP_FULL)
-    voxels = c.dense_stats()["voxels"]
+    from loam_velodyne_b200 import api
+    _, _, _, fulls, twists = replay_run(args.sweeps)
+    c, voxels = dense_ctx(fulls, args.leaf)
     n_target = c.dense_target_build(None, 2, (0.0, 0.0, 0.0))
     centre = np.asarray(twists[-1][3:], np.float64)
 
@@ -96,19 +67,14 @@ def main():
             except api.LoamB200Error as e:
                 refused[name] = {"dims": [int(d) for d in dims], "padded": padded,
                                  "padded_cells": int(np.prod(padded)), "error": str(e)}
-    times = {name: [] for name in cases}
-    for rep in range(args.reps + 1):
-        for name, (lo, dims, md, _) in cases.items():
-            c.profile(True)
-            c.dense_distance_field(lo, dims, md, download=False)
-            if rep:
-                times[name].append(c.profile_get()["dense"][0])
+    times = profiled(c, {name: (lambda lo=lo, dims=dims, md=md: c.dense_distance_field(lo, dims, md, download=False))
+                         for name, (lo, dims, md, _) in cases.items()}, args.reps)
     builds = {}
     for name, (lo, dims, md, pad) in cases.items():
-        med = float(np.median(times[name]))
+        med = float(np.median(times[name].gpu_ms))
         cells = int(np.prod(dims))
         nbytes = algorithmic_bytes(dims, pad)
-        builds[name] = {"dims": [int(d) for d in dims], "pad": pad, "cells": cells, "gpu_ms": stats(times[name]),
+        builds[name] = {"dims": [int(d) for d in dims], "pad": pad, "cells": cells, "gpu_ms": stats(times[name].gpu_ms),
                         "cells_per_s": round(cells / (med * 1e-3), 1), "algorithmic_bytes": nbytes,
                         "algorithmic_tb_per_s": round(nbytes / (med * 1e-3) / 1e12, 3),
                         "fraction_of_hbm": round(nbytes / (med * 1e-3) / 1e12 / HBM_TBPS, 3)}
@@ -126,16 +92,12 @@ def main():
         pts = torch.zeros((n, 4), dtype=torch.float32, device="cuda")
         pts[:, :3] = lo_m + torch.rand((n, 3), generator=g, device="cuda") * ext_m
         torch.cuda.synchronize()
-        t = []
-        for rep in range(args.reps + 1):
-            c.profile(True)
-            d, _ = c.dense_distance_query(pts.data_ptr(), on_device=True, n=n, gradient=True)
-            if rep:
-                t.append(c.profile_get()["dense"][0])
-        med = float(np.median(t))
-        queries[str(n)] = {"gpu_ms": stats(t), "points_per_s": round(n / (med * 1e-3), 1),
-                           "defined_fraction": round(float(np.isfinite(d).mean()), 4)}
-        del pts
+        q = profiled(c, {"query": lambda: c.dense_distance_query(pts.data_ptr(), on_device=True, n=n, gradient=True)},
+                     args.reps)["query"]
+        med = float(np.median(q.gpu_ms))
+        queries[str(n)] = {"gpu_ms": stats(q.gpu_ms), "points_per_s": round(n / (med * 1e-3), 1),
+                           "defined_fraction": round(float(np.isfinite(q.out[0]).mean()), 4)}
+        del pts, q
     c.close()
 
     print(json.dumps({

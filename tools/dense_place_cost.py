@@ -2,8 +2,7 @@
 """What place recognition and global relocalisation in the whole-run voxel map cost.
 
 Workloads, with the card's name and power limit read in the same run:
-  * the config-3 map of tools/dense_raycast_cost.py (HDL-64E 64 x 2048 sweeps against a 1 M-point surrounding map,
-    --sweeps sweeps replayed at --leaf, target radius 2);
+  * the replayed hdl64_1m map of tools/dense_cost.py, --sweeps sweeps at --leaf, target radius 2;
   * the route map of tests/test_dense_place.py (HDL-64E 64 x 512 static sweeps every 4 m along 180 m of streets,
     leaf --leaf), places every 4 m.
 Reported (GPU time from CUDA-event profiling, family "dense", median / min / max over --reps rounds after a warm-up):
@@ -20,7 +19,6 @@ from __future__ import annotations
 
 import argparse
 import json
-import math
 import os
 import re
 import subprocess
@@ -29,26 +27,10 @@ import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.dont_write_bytecode = True
+from dense_cost import ROOT, dense_ctx, gpu_info, profiled, replay_run, require_cuda, stats  # noqa: E402
 
-
-def stats(v):
-    return {"median": round(float(np.median(v)), 4), "min": round(float(np.min(v)), 4),
-            "max": round(float(np.max(v)), 4)}
-
-
-def timed(c, fn, reps):
-    out = []
-    for rep in range(reps + 1):
-        c.profile(True)
-        fn()
-        if rep:
-            out.append(c.profile_get()["dense"][0])
-    return stats(out)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def ptxas():
@@ -74,31 +56,12 @@ def main():
     ap.add_argument("--ptxas", action="store_true")
     args = ap.parse_args()
 
-    import torch
-    from dense_raycast_cost import gpu_info
+    require_cuda("dense_place_cost")
     from loam_velodyne_b200 import api, synth
     import align_reference as ar
     from test_dense_place import route
-    if not torch.cuda.is_available():
-        raise SystemExit("dense_place_cost: no CUDA device (nothing here runs on the CPU)")
-    scene = synth.make_scene()
-    lidar = synth.Lidar.hdl64()
-    corner, surf = synth.make_map(scene, 1_000_000)
-    seq = api.Pipeline()
-    seq.seed_map(corner, surf)
-    fulls, twists = [], []
-    for i in range(args.sweeps):
-        seq.sweep(*synth.make_sweep(scene, lidar, i, yaw_rate=math.radians(5.0)))
-        fulls.append(seq.mapping.cloud("full"))
-        twists.append(seq.mapping.twist("aft"))
-    seq.sync()
-    del seq
-
-    c = api.Ctx(0)
-    c.dense_enable(args.leaf)
-    for f in fulls:
-        c.cloud_upload(api.C_MAP_FULL, f)
-        c.dense_insert(api.C_MAP_FULL)
+    scene, lidar, sweeps, fulls, twists = replay_run(args.sweeps)
+    c, _ = dense_ctx(fulls, args.leaf)
     n_target = c.dense_target_build(None, 2, (0.0, 0.0, 0.0))
     prm = api.PlaceParams.default()
     elev = np.linspace(lidar.lower_deg, lidar.upper_deg, lidar.n_rings)
@@ -109,35 +72,34 @@ def main():
         return np.stack([centre[0] + rng.uniform(-20, 20, k), np.full(k, centre[1]),
                          centre[2] + rng.uniform(-20, 20, k)], 1).astype(np.float32)
 
+    def timed(ctx, fn):
+        return stats(profiled(ctx, {"call": fn}, args.reps)["call"].gpu_ms)
+
     c.dense_raycast(api.lidar_rays(elev, 8), twists[0])  # the ray index, outside the timed builds
     build = {}
     for n_az in (360, 720):
         rays = api.lidar_rays(elev, n_az)
         for k in (100, 1000, 10000):
             p = positions(k)
-            build[f"{k}_candidates_{rays.shape[0]}_rays"] = timed(c, lambda: c.dense_place_build(p, rays, prm),
-                                                                  args.reps)
+            build[f"{k}_candidates_{rays.shape[0]}_rays"] = timed(c, lambda: c.dense_place_build(p, rays, prm))
     query = {}
-    q, _ = synth.make_sweep(scene, lidar, args.sweeps // 2, yaw_rate=math.radians(5.0))
+    q = sweeps[args.sweeps // 2][0]
     for k in (1000, 10000, 100000):
         c.dense_place_build(positions(k), api.lidar_rays(elev, 360), prm)
-        query[f"{k}_candidates"] = timed(c, lambda: c.dense_place_query(q, top_m=api.PLACE_TOP_M), args.reps)
+        query[f"{k}_candidates"] = timed(c, lambda: c.dense_place_query(q, top_m=api.PLACE_TOP_M))
     c.close()
 
     # the route map
     small = synth.Lidar.hdl64(512)
-    r = api.Ctx(0)
-    r.dense_enable(args.leaf)
     pos, yaw = route(4.0)
-    for k in range(pos.shape[0]):
-        r.cloud_upload(api.C_MAP_FULL, ar.static_sweep(scene, small, np.array([0.0, yaw[k], 0.0, *pos[k]]), seed=k)[1])
-        r.dense_insert(api.C_MAP_FULL)
+    r, _ = dense_ctx((ar.static_sweep(scene, small, np.array([0.0, yaw[k], 0.0, *pos[k]]), seed=k)[1]
+                      for k in range(pos.shape[0])), args.leaf)
     n_route = r.dense_target_build(None, 2, (0.0, 0.0, 0.0))
     traj, _ = route(1.0)
     places = api.thin_trajectory(traj, api.PLACE_SPACING)
     rays = api.lidar_rays(np.linspace(small.lower_deg, small.upper_deg, small.n_rings), 360)
     r.dense_raycast(rays[:8], np.zeros(6))
-    route_build = timed(r, lambda: r.dense_place_build(places, rays, prm), args.reps)
+    route_build = timed(r, lambda: r.dense_place_build(places, rays, prm))
     truth = np.array([0.0, 2.0, 0.0, 31.0, 0.0, 0.8], np.float32)
     qs = ar.static_sweep(scene, small, truth.astype(np.float64), seed=77)[0]
     grid = api.reloc_grid(truth)

@@ -1,10 +1,8 @@
 #!/usr/bin/env python
 """What ray casting the whole-run voxel map costs.
 
-Workload: the map of tools/dense_align_cost.py -- BASELINE config 3 (HDL-64E 64 x 2048 sweeps against a 1 M-point
-surrounding map), --sweeps sweeps through the pipeline, their registered clouds replayed into a kernel-level context
-with the whole-run map at --leaf, and the target built from it (radius 2).  Reported, with the card's name and power
-limit read in the same run:
+Workload: the replayed hdl64_1m map (tools/dense_cost.py), --sweeps sweeps at --leaf, and the target built from it
+(radius 2).  Reported, with the card's name and power limit read in the same run:
   * the first cast after the build (64 x 2048 grid, max_range 100 m): GPU time including the ray index build
     (CUDA-event profiling, family "dense"), over --reps builds;
   * later casts of a 64 x 2048 lidar_rays grid at max_range 50, 100 and 200 m, and of a 131 k-point sweep's own
@@ -18,40 +16,12 @@ from __future__ import annotations
 
 import argparse
 import json
-import math
-import os
 import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
 sys.dont_write_bytecode = True
-
-
-def gpu_info():
-    try:
-        import pynvml
-        pynvml.nvmlInit()
-        h = pynvml.nvmlDeviceGetHandleByIndex(0)
-        name = pynvml.nvmlDeviceGetName(h)
-        return {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": round(pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0, 1)}
-    except Exception:
-        import subprocess
-        try:
-            out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                                 stdout=subprocess.PIPE, text=True, check=True).stdout.strip().splitlines()[0]
-            name, limit = (s.strip() for s in out.split(","))
-            return {"name": name, "power_limit": limit}
-        except Exception:
-            import torch
-            return {"name": torch.cuda.get_device_name(0), "power_limit_w": None}
-
-
-def stats(v):
-    return {"median": round(float(np.median(v)), 4), "min": round(float(np.min(v)), 4),
-            "max": round(float(np.max(v)), 4)}
+from dense_cost import dense_ctx, gpu_info, profiled, replay_run, require_cuda, stats  # noqa: E402
 
 
 def main():
@@ -61,34 +31,15 @@ def main():
     ap.add_argument("--reps", type=int, default=15)
     args = ap.parse_args()
 
-    import torch
-    from loam_velodyne_b200 import api, synth
-    if not torch.cuda.is_available():
-        raise SystemExit("dense_raycast_cost: no CUDA device (nothing here runs on the CPU)")
-    scene = synth.make_scene()
-    lidar = synth.Lidar.hdl64()
-    corner, surf = synth.make_map(scene, 1_000_000)
-    seq = api.Pipeline()
-    seq.seed_map(corner, surf)
-    fulls, twists = [], []
-    for i in range(args.sweeps):
-        seq.sweep(*synth.make_sweep(scene, lidar, i, yaw_rate=math.radians(5.0)))
-        fulls.append(seq.mapping.cloud("full"))
-        twists.append(seq.mapping.twist("aft"))
-    seq.sync()
-    del seq
-
-    c = api.Ctx(0)
-    c.dense_enable(args.leaf)
-    for f in fulls:
-        c.cloud_upload(api.C_MAP_FULL, f)
-        c.dense_insert(api.C_MAP_FULL)
-    voxels = c.dense_stats()["voxels"]
+    require_cuda("dense_raycast_cost")
+    from loam_velodyne_b200 import api
+    _, lidar, sweeps, fulls, twists = replay_run(args.sweeps)
+    c, voxels = dense_ctx(fulls, args.leaf)
 
     k = args.sweeps // 2
     pose = twists[k]
     grid = api.lidar_rays(np.linspace(lidar.lower_deg, lidar.upper_deg, lidar.n_rings), 2048)
-    pts, _ = synth.make_sweep(scene, lidar, k, yaw_rate=math.radians(5.0))
+    pts = sweeps[k][0]
 
     first = []
     for rep in range(args.reps + 1):
@@ -101,15 +52,8 @@ def main():
 
     cases = {"grid_50m": (grid, 50.0), "grid_100m": (grid, 100.0), "grid_200m": (grid, 200.0),
              "sweep_100m": (pts, 100.0)}
-    later = {name: [] for name in cases}
-    hits = {}
-    for rep in range(args.reps + 1):
-        for name, (rays, mx) in cases.items():
-            c.profile(True)
-            r, _ = c.dense_raycast(rays, pose, 0.0, mx)
-            if rep:
-                later[name].append(c.profile_get()["dense"][0])
-            hits[name] = round(float(np.isfinite(r).mean()), 4)
+    later = profiled(c, {name: (lambda rays=rays, mx=mx: c.dense_raycast(rays, pose, 0.0, mx))
+                         for name, (rays, mx) in cases.items()}, args.reps)
     c.close()
 
     print(json.dumps({
@@ -117,7 +61,8 @@ def main():
                     f" cast from sweep {k}'s mapped pose: a 64 x 2048 grid, sweep {k}'s own {pts.shape[0]} points",
         "voxels": voxels, "target_voxels": n_target, "reps": args.reps, "ray_index_bytes": index_bytes,
         "first_cast_with_index_gpu_ms": stats(first),
-        "cast_gpu_ms": {name: stats(v) for name, v in later.items()}, "hit_fraction": hits,
+        "cast_gpu_ms": {name: stats(p.gpu_ms) for name, p in later.items()},
+        "hit_fraction": {name: round(float(np.isfinite(p.out[0]).mean()), 4) for name, p in later.items()},
         "gpu": gpu_info(),
     }))
 

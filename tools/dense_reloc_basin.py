@@ -21,11 +21,10 @@ import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.dont_write_bytecode = True
+from dense_cost import ROOT, dense_ctx, gpu_info, require_cuda  # noqa: E402
+
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def main():
@@ -36,20 +35,16 @@ def main():
     yaws = [float(v) for v in args.yaw.split(",")]
     metres = [float(v) for v in args.metres.split(",")]
 
+    require_cuda("dense_reloc_basin")
     import align_reference as ar
-    from dense_align_cost import gpu_info
-    from loam_velodyne_b200 import api, synth
+    from loam_velodyne_b200 import synth
     from test_align_reference import BAR_DEG, BAR_M, HELD_OUT, MAP_TWISTS, lidars
 
     scene = synth.make_scene()
     out = {}
     for sensor, lidar in lidars().items():
         for leaf in (0.1, 0.2):
-            c = api.Ctx(0)
-            c.dense_enable(leaf)
-            for k, tw in enumerate(MAP_TWISTS):
-                c.cloud_upload(api.C_MAP_FULL, ar.static_sweep(scene, lidar, tw, seed=k)[1])
-                c.dense_insert(api.C_MAP_FULL)
+            c, _ = dense_ctx([ar.static_sweep(scene, lidar, tw, seed=k)[1] for k, tw in enumerate(MAP_TWISTS)], leaf)
             c.dense_target_build(None, 2)
             ok = {(y, m): 0 for y in yaws for m in metres}
             runs = {(y, m): 0 for y in yaws for m in metres}

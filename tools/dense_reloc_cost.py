@@ -1,10 +1,8 @@
 #!/usr/bin/env python
 """What relocalising a sweep in the whole-run voxel map costs.
 
-Workload: the map of tools/dense_align_cost.py -- BASELINE config 3 (HDL-64E 64 x 2048 sweeps against a 1 M-point
-surrounding map), --sweeps sweeps through the pipeline, their registered clouds replayed into a kernel-level context
-with the whole-run map at --leaf, target built at normals radius 2.  Reported, with the card's name and power limit
-read in the same run:
+Workload: the replayed hdl64_1m map (tools/dense_cost.py), --sweeps sweeps at --leaf, target built at normals radius
+2.  Reported, with the card's name and power limit read in the same run:
   * the score pass (dense_score at radius 3): GPU time of its launches (CUDA-event profiling, family "dense") against
     k (1 k, 10 k, 100 k poses near the mapped pose) at n = 32 k points, and against n (the 131 k-point sweep strided to
     8 k, 32 k and 131 k points) at k = 10 k; median, min and max over --reps after one warm-up;
@@ -30,12 +28,8 @@ import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.dont_write_bytecode = True
-
-from dense_align_cost import gpu_info, stats  # noqa: E402
+from dense_cost import ROOT, dense_ctx, gpu_info, profiled, replay_run, require_cuda, stats  # noqa: E402
 
 
 class BaselineAlign:
@@ -77,32 +71,14 @@ def main():
     ap.add_argument("--baseline-lib", default=None)
     args = ap.parse_args()
 
-    import torch
-    from loam_velodyne_b200 import api, synth
-    if not torch.cuda.is_available():
-        raise SystemExit("dense_reloc_cost: no CUDA device (nothing here runs on the CPU)")
-    scene = synth.make_scene()
-    lidar = synth.Lidar.hdl64()
-    corner, surf = synth.make_map(scene, 1_000_000)
-    seq = api.Pipeline()
-    seq.seed_map(corner, surf)
-    fulls, twists = [], []
-    for i in range(args.sweeps):
-        seq.sweep(*synth.make_sweep(scene, lidar, i, yaw_rate=math.radians(5.0)))
-        fulls.append(seq.mapping.cloud("full"))
-        twists.append(seq.mapping.twist("aft"))
-    seq.sync()
-    del seq
-
-    c = api.Ctx(0)
-    c.dense_enable(args.leaf)
-    for f in fulls:
-        c.cloud_upload(api.C_MAP_FULL, f)
-        c.dense_insert(api.C_MAP_FULL)
+    require_cuda("dense_reloc_cost")
+    from loam_velodyne_b200 import api
+    _, _, sweeps, fulls, twists = replay_run(args.sweeps)
+    c, _ = dense_ctx(fulls, args.leaf)
     n_target = c.dense_target_build(None, 2, (0.0, 0.0, 0.0))
 
     k = args.sweeps // 2
-    pts, _ = synth.make_sweep(scene, lidar, k, yaw_rate=math.radians(5.0))
+    pts = sweeps[k][0]
     mapped = twists[k]
     rng = np.random.RandomState(5)
 
@@ -114,13 +90,7 @@ def main():
         return (mapped + d).astype(np.float32)
 
     def gpu_ms(fn):
-        out = []
-        for rep in range(args.reps + 1):
-            c.profile(True)
-            fn()
-            if rep:
-                out.append(c.profile_get()["dense"][0])
-        return stats(out)
+        return stats(profiled(c, {"call": fn}, args.reps)["call"].gpu_ms)
 
     strided = {n: pts[::max(1, pts.shape[0] // n)][:n] for n in (8192, 32768, pts.shape[0])}
     poses = {kk: near(kk) for kk in (1000, 10000, 100000)}

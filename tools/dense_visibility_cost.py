@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """What the visibility pass of the whole-run voxel map costs the streaming pipeline.
 
-Workload: BASELINE config 3 (HDL-64E 64 x 2048 sweeps against a 1 M-point surrounding map), the whole-run map at
---leaf in both arms.  The streaming throughput is timed with the pass off and on (--h-res / --v-res / --margin), in
-alternating windows of --steps sweeps on a fresh pipeline each (after --warmup sweeps), repeated until each arm has
---min-seconds of timed windows (at least three); median, min and max window are reported per arm.  A separate run
-times the pass's kernels alone: the registered clouds and poses of the same stream are replayed into a kernel-level
-context, with CUDA-event profiling (family "dense") switched on around each dense_observe only.  The hash table's size
-is read from the library at the end of each arm's last window and of the replay.  Prints one JSON line.
+Workload: hdl64_1m streaming (tools/dense_cost.py), the whole-run map at --leaf in both arms.  The streaming throughput
+is timed with the pass off and on (--h-res / --v-res / --margin), in alternating windows of --steps sweeps on a fresh
+pipeline each (after --warmup sweeps), repeated until each arm has --min-seconds of timed windows (at least three);
+median, min and max window are reported per arm.  A separate run times the pass's kernels alone: the registered clouds
+and poses of the same stream are replayed into a kernel-level context, with CUDA-event profiling (family "dense")
+switched on around each dense_observe only.  The hash table's size is read from the library at the end of each arm's
+last window and of the replay.  Prints one JSON line.
 
     python tools/dense_visibility_cost.py [--steps 50 --warmup 5 --leaf 0.1 --min-seconds 0.6]
 """
@@ -15,29 +15,12 @@ from __future__ import annotations
 
 import argparse
 import json
-import math
-import os
 import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
 sys.dont_write_bytecode = True
-
-
-def gpu_info():
-    try:
-        import pynvml
-        pynvml.nvmlInit()
-        h = pynvml.nvmlDeviceGetHandleByIndex(0)
-        name = pynvml.nvmlDeviceGetName(h)
-        return {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": round(pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0, 1)}
-    except Exception:
-        import torch
-        return {"name": torch.cuda.get_device_name(0), "power_limit_w": None}
+from dense_cost import gpu_info, hdl64_1m, require_cuda, stream_windows  # noqa: E402
 
 
 def main():
@@ -52,69 +35,24 @@ def main():
     ap.add_argument("--max-windows", type=int, default=40)
     args = ap.parse_args()
 
-    import torch
-    from loam_velodyne_b200 import api, synth
-    if not torch.cuda.is_available():
-        raise SystemExit("dense_visibility_cost: no CUDA device (nothing here runs on the CPU)")
-    scene = synth.make_scene()
-    lidar = synth.Lidar.hdl64()
-    corner, surf = synth.make_map(scene, 1_000_000)
-    n = args.warmup + args.steps
-    sweeps = [synth.make_sweep(scene, lidar, i, yaw_rate=math.radians(5.0)) for i in range(n)]
-    d_sweeps = [torch.from_numpy(p).to("cuda:0") for p, _ in sweeps]
-    torch.cuda.synchronize()
+    require_cuda("dense_visibility_cost")
+    from loam_velodyne_b200 import api
+    _, _, seed, sweeps = hdl64_1m(args.warmup + args.steps)
 
     def pipeline(vis):
         p = api.Pipeline()
-        p.seed_map(corner, surf)
+        p.seed_map(*seed)
         p.mapping.enable_dense_map(args.leaf)
         if vis:
             p.mapping.enable_dense_visibility(args.h_res, args.v_res, args.margin)
         return p
 
-    def window(vis):
-        p = pipeline(vis)
+    def probe(p, vis):
+        return dict(p.mapping.dense_stats(), table_slots=p.mapping.dense_table_slots())
 
-        def run(lo, hi):
-            got = 0
-            for i in range(lo, hi):
-                p.submit(ring_sizes=sweeps[i][1], device_ptr=d_sweeps[i].data_ptr())
-                if p.collect(wait=False) is not None:
-                    got += 1
-            while got < hi - lo:
-                p.collect(wait=True)
-                got += 1
-            p.sync()
-
-        run(0, args.warmup)
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        run(args.warmup, n)  # ends with every stage (and the map's pass and insertion) finished on the GPU
-        torch.cuda.synchronize()
-        el = time.perf_counter() - t0
-        stats = dict(p.mapping.dense_stats(), table_slots=p.mapping.dense_table_slots())
-        del p
-        return el, stats
-
-    windows = {False: [], True: []}
-    last = {}
-    while True:
-        for vis in (False, True):
-            el, stats = window(vis)
-            windows[vis].append(el)
-            last[vis] = stats
-        done = [sum(windows[v]) >= args.min_seconds and len(windows[v]) >= 3 for v in (False, True)]
-        if all(done) or len(windows[True]) >= args.max_windows:
-            break
-
-    def arm(els):
-        s = sorted(els)
-        sps = [args.steps / e for e in s]
-        return {"sweeps_per_s_median": round(args.steps / s[len(s) // 2], 1), "sweeps_per_s_min": round(min(sps), 1),
-                "sweeps_per_s_max": round(max(sps), 1), "windows": len(s),
-                "window_ms_min_median_max": [round(1e3 * s[0], 2), round(1e3 * s[len(s) // 2], 2), round(1e3 * s[-1], 2)]}
-
-    off, on = arm(windows[False]), arm(windows[True])
+    rates, probes = stream_windows(args, sweeps, pipeline, (False, True), probe)
+    off, on = rates[False], rates[True]
+    last = {vis: probes[vis][-1] for vis in (False, True)}
 
     # the registered clouds and optimised poses of the stream, one sweep at a time
     seq = pipeline(True)

@@ -451,6 +451,50 @@ int loam_b200_debug_dense_table_slots(loam_b200_ctx* ctx, long long* out);
 int loam_b200_debug_dense_carve_index(loam_b200_ctx* ctx, uint64_t* rows, long long cap, long long* n_out);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Whole-run voxel map snapshots and merging (csrc/densemap.cuh, DESIGN.md "Snapshots and merging"): the accumulator's
+ * own state, saved exactly and added back into a map -- resume a stopped run, extend one session's map with another's
+ * under the rigid transform dense_relocalize(_global) found, or make a coarser copy.  Not on the per-sweep path.
+ *   snapshot: every stored voxel in ascending key order with the fields of its table entry: key (the key codec of
+ *           DESIGN.md §5.1: (v_z + 2^20) << 42 | (v_y + 2^20) << 21 | (v_x + 2^20)), count, hits, misses and the four
+ *           fp64 sums (x, y, z, intensity) as sums[4 i .. 4 i + 3].  keys, hits and misses may be NULL; counts and sums
+ *           may not once voxels are returned (LOAM_B200_ERR_ARG).  *n_out = number of voxels, LOAM_B200_ERR_CAPACITY
+ *           when it exceeds cap; not enabled: an empty map.  Synchronous, after everything enqueued on the map's
+ *           stream.  (float)(sums / count) equals loam_b200_dense_export's centroids bit for bit; counts, hits and
+ *           misses equal loam_b200_dense_export_filtered(+inf)'s.
+ *   merge:  add n entries (counts, hits, misses, sums as the snapshot returns them; no keys, no leaf) into the map,
+ *           optionally under `pose` (NULL: as stored).  fp64 without FMA, each operation rounded on its own:
+ *             S' = S when pose is NULL; otherwise (Sx, Sy, Sz) rotated by rotZ, then rotX, then rotY (as
+ *               loam_b200_dense_raycast, with std::cos / std::sin in double of the pose's float angles) and
+ *               (double)count * (double)pos_a added per axis; the intensity sum is unchanged.
+ *             destination voxel: c_a = (float)(S'_a / (double)count), the key of the map's rule (floorf(c_a * (1.0f /
+ *               leaf)) in fp32, the map's current leaf).  So an entry's voxel follows from its centroid: a snapshot
+ *               merges into a map of another leaf (into a larger leaf: a coarse copy).  A centroid that is not finite
+ *               or whose voxel lies outside the key range is skipped; its count is added to `skipped`.
+ *             entries with one destination are combined in ascending input index: P = ((0.0 + S'_i1) + S'_i2) + ...;
+ *               counts add (uint32); hits and misses each add with saturation at 65535.
+ *             a stored voxel gets S + P, count + the group's count and the saturating sums of its hits and misses; a
+ *               new voxel is admitted in ascending key order while the map is under max_voxels (as the insertion
+ *               admits one; the count of a group refused is added to `dropped`) with P, the group's count and evidence.
+ *               A merge adds no hit of its own: the evidence carried in is the evidence.
+ *           Counts add in uint32 as the insertion's do; neither guards against overflow.  With carve mode on, the
+ *           voxels admitted enter its occupancy index.  Runs on the map's stream after everything enqueued on the
+ *           context; everything enqueued on the context afterwards waits for it.  A target, its ray index, distance
+ *           field and place database built earlier do not change.
+ *           Every check runs before anything is uploaded, so a refused call changes nothing: LOAM_B200_ERR_ARG for
+ *           n < 0, a NULL array with n > 0, an entry with count 0 or hits 0 (every stored voxel has a hit), a sum that
+ *           is not finite, or a pose with a non-finite angle or position; LOAM_B200_ERR_STATE without the map or on a
+ *           sharded context.  n == 0 launches nothing.
+ *   Resume: a snapshot merged into an empty map of the same leaf with pose NULL reproduces it bit for bit -- each
+ *   entry lands in its own voxel (a centroid lies between its points and floorf is monotone), and 0.0 + S == S since
+ *   a stored sum is never -0.0 -- so inserting the remaining sweeps afterwards gives the map of a run that never
+ *   stopped.  A zero pose gives the same bits as NULL on snapshot input.  Launches count under LOAM_B200_K_DENSE.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int loam_b200_dense_snapshot(loam_b200_ctx* ctx, uint64_t* keys, uint32_t* counts, uint16_t* hits, uint16_t* misses,
+                             double* sums, int cap, int* n_out);
+int loam_b200_dense_merge(loam_b200_ctx* ctx, const uint32_t* counts, const uint16_t* hits, const uint16_t* misses,
+                          const double* sums, int n, const loam_b200_pose* pose);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Alignment against the whole-run voxel map (csrc/densemap.cuh, DESIGN.md "Alignment against the whole-run voxel map"):
  * point-to-plane Gauss-Newton of a cloud against a device-resident target of voxel centroids and normals, for
  * relocalisation in a map built earlier, drift checks of a mapped pose, or placing another sensor's or session's sweeps

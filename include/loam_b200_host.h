@@ -116,6 +116,14 @@ int loam_b200_map_dense_export_filtered(void* h, double max_miss_ratio, float* x
  * arguments, capacity rule and in-flight rule as loam_b200_map_dense_export_filtered, viewpoint = 3 doubles. */
 int loam_b200_map_dense_export_normals(void* h, double max_miss_ratio, int radius, const double* viewpoint,
                                        float* xyzi, unsigned int* counts, float* normals, int cap, int* n_out);
+/* snapshots and merging (BasicLaserMapping::denseMapSnapshot / mergeDenseMap, include/loam_b200.h "Whole-run voxel
+ * map snapshots and merging"), same in-flight rule.  snapshot: as loam_b200_dense_snapshot (keys, hits, misses may be
+ * NULL; capacity rule of the exports).  merge: n entries as loam_b200_dense_merge, pose6 = twist (rot_x, rot_y, rot_z,
+ * x, y, z) or NULL. */
+int loam_b200_map_dense_snapshot(void* h, unsigned long long* keys, unsigned int* counts, unsigned short* hits,
+                                 unsigned short* misses, double* sums, int cap, int* n_out);
+int loam_b200_map_dense_merge(void* h, const unsigned int* counts, const unsigned short* hits,
+                              const unsigned short* misses, const double* sums, int n, const float* pose6);
 /* test query: loam_b200_debug_dense_table_slots of the mapping object's context (BasicLaserMapping::denseTableSlots) */
 int loam_b200_map_debug_dense_table_slots(void* h, long long* out);
 /* alignment against the whole-run map (BasicLaserMapping::buildDenseTarget / loadDenseTarget / alignToDenseTarget,

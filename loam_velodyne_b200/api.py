@@ -216,6 +216,8 @@ def lib():
         "loam_b200_dense_export_normals": (C.c_int, [vp, C.c_double, C.c_int, _D, _F, _U, _F, C.c_int, _I]),
         "loam_b200_debug_dense_table_slots": (C.c_int, [vp, _LL]),
         "loam_b200_debug_dense_carve_index": (C.c_int, [vp, C.POINTER(C.c_uint64), C.c_longlong, _LL]),
+        "loam_b200_dense_snapshot": (C.c_int, [vp, C.POINTER(C.c_uint64), _U, _U16, _U16, _D, C.c_int, _I]),
+        "loam_b200_dense_merge": (C.c_int, [vp, _U, _U16, _U16, _D, C.c_int, C.POINTER(Pose)]),
         "loam_b200_dense_target_build": (C.c_int, [vp, C.c_double, C.c_int, _D, _I]),
         "loam_b200_dense_target_load": (C.c_int, [vp, C.c_float, _F, _F, C.c_int]),
         "loam_b200_dense_align_iterate": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int,
@@ -296,6 +298,8 @@ def lib():
         "loam_b200_map_dense_export_filtered": (C.c_int, [vp, C.c_double, _F, _U, _U16, _U16, C.c_int, _I]),
         "loam_b200_map_dense_export_normals": (C.c_int, [vp, C.c_double, C.c_int, _D, _F, _U, _F, C.c_int, _I]),
         "loam_b200_map_debug_dense_table_slots": (C.c_int, [vp, _LL]),
+        "loam_b200_map_dense_snapshot": (C.c_int, [vp, C.POINTER(C.c_uint64), _U, _U16, _U16, _D, C.c_int, _I]),
+        "loam_b200_map_dense_merge": (C.c_int, [vp, _U, _U16, _U16, _D, C.c_int, _F]),
         "loam_b200_map_dense_target_build": (C.c_int, [vp, C.c_double, C.c_int, _D, _I]),
         "loam_b200_map_dense_target_load": (C.c_int, [vp, C.c_float, _F, _F, C.c_int]),
         "loam_b200_map_dense_align": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.c_int, _F, _I, _F]),
@@ -682,6 +686,7 @@ class Ctx:
     # ---- whole-run voxel map (include/loam_b200.h "Whole-run voxel map")
     def dense_enable(self, leaf, max_voxels=DENSE_MAX_VOXELS):
         self._ck(self.L.loam_b200_dense_enable(self.h, np.float32(leaf), int(max_voxels)), "dense_enable")
+        self.dense_leaf = np.float32(leaf)
 
     def dense_insert(self, slot):
         """Accumulate the cloud in `slot` (fill it with cloud_upload)."""
@@ -747,6 +752,21 @@ class Ctx:
 
     def dense_clear(self):
         self._ck(self.L.loam_b200_dense_clear(self.h), "dense_clear")
+
+    # ---- snapshots and merging (include/loam_b200.h "Whole-run voxel map snapshots and merging")
+    def dense_snapshot(self):
+        """The exact state of every stored voxel in ascending key order: a dict of "keys" (N uint64), "counts" (N
+        uint32), "hits", "misses" (N uint16), "sums" (N x 4 float64: x, y, z, intensity) and "leaf" (the map's leaf)."""
+        return _dense_snapshot(lambda *a: self.L.loam_b200_dense_snapshot(self.h, *a), self.dense_stats()["voxels"],
+                               getattr(self, "dense_leaf", None), lambda rc: self._ck(rc, "dense_snapshot"))
+
+    def dense_merge(self, snap, twist6=None):
+        """Add a snapshot's entries into the map, as stored (twist6 None) or under the rigid transform twist6 = (rot_x,
+        rot_y, rot_z, x, y, z); each entry's voxel is that of its transformed centroid at this map's leaf."""
+        a = _merge_arrays(snap)
+        p = make_pose(twist6) if twist6 is not None else None
+        self._ck(self.L.loam_b200_dense_merge(self.h, *_merge_ptrs(a), C.byref(p) if p is not None else None),
+                 "dense_merge")
 
     # ---- alignment against the whole-run voxel map (include/loam_b200.h "Alignment against the whole-run voxel map")
     def dense_target_build(self, max_miss_ratio=None, radius=1, viewpoint=(0.0, 0.0, 0.0)):
@@ -999,6 +1019,62 @@ def _dense_export_normals(fn, max_miss_ratio, radius, viewpoint, n, ck):
     return pts[:k].copy(), cnt[:k].copy(), nrm[:k].copy()
 
 
+def _dense_snapshot(fn, n, leaf, ck):
+    keys = np.zeros(max(n, 1), np.uint64)
+    cnt = np.zeros(max(n, 1), np.uint32)
+    hits = np.zeros(max(n, 1), np.uint16)
+    misses = np.zeros(max(n, 1), np.uint16)
+    sums = np.zeros((max(n, 1), 4), np.float64)
+    got = C.c_int(0)
+    ck(fn(keys.ctypes.data_as(C.POINTER(C.c_uint64)), cnt.ctypes.data_as(_U), hits.ctypes.data_as(_U16),
+          misses.ctypes.data_as(_U16), sums.ctypes.data_as(_D), n, C.byref(got)))
+    k = got.value
+    return {"leaf": None if leaf is None else np.float32(leaf), "keys": keys[:k].copy(), "counts": cnt[:k].copy(),
+            "hits": hits[:k].copy(), "misses": misses[:k].copy(), "sums": sums[:k].copy()}
+
+
+def _merge_arrays(snap):
+    """(counts uint32, hits uint16, misses uint16, sums N x 4 float64) of a snapshot dict, contiguous."""
+    cnt = np.ascontiguousarray(snap["counts"], np.uint32).reshape(-1)
+    hits = np.ascontiguousarray(snap["hits"], np.uint16).reshape(-1)
+    misses = np.ascontiguousarray(snap["misses"], np.uint16).reshape(-1)
+    sums = np.ascontiguousarray(snap["sums"], np.float64).reshape(-1, 4)
+    if not hits.shape[0] == misses.shape[0] == sums.shape[0] == cnt.shape[0]:
+        raise ValueError("dense_merge: the snapshot's arrays differ in length")
+    return cnt, hits, misses, sums
+
+
+def _merge_ptrs(arrays):
+    cnt, hits, misses, sums = arrays
+    return (cnt.ctypes.data_as(_U), hits.ctypes.data_as(_U16), misses.ctypes.data_as(_U16), sums.ctypes.data_as(_D),
+            cnt.shape[0])
+
+
+DENSE_SNAPSHOT_FORMAT = 1  # version of the .npz layout of save_dense_snapshot
+
+
+def save_dense_snapshot(path, snap):
+    """Write a snapshot (Ctx.dense_snapshot / LaserMapping.dense_map_snapshot) to a plain .npz file: the five arrays,
+    the leaf and a format version; no pickled objects."""
+    leaf = snap.get("leaf")
+    np.savez(path, format=np.int64(DENSE_SNAPSHOT_FORMAT), leaf=np.float32(np.nan if leaf is None else leaf),
+             keys=np.asarray(snap["keys"], np.uint64), counts=np.asarray(snap["counts"], np.uint32),
+             hits=np.asarray(snap["hits"], np.uint16), misses=np.asarray(snap["misses"], np.uint16),
+             sums=np.asarray(snap["sums"], np.float64).reshape(-1, 4))
+
+
+def load_dense_snapshot(path):
+    """Read a file written by save_dense_snapshot -> the snapshot dict (ValueError on another format version)."""
+    with np.load(path, allow_pickle=False) as z:
+        version = int(z["format"])
+        if version != DENSE_SNAPSHOT_FORMAT:
+            raise ValueError(f"load_dense_snapshot: format {version}, expected {DENSE_SNAPSHOT_FORMAT}")
+        leaf = np.float32(z["leaf"])
+        return {"leaf": None if np.isnan(leaf) else leaf, "keys": z["keys"].astype(np.uint64),
+                "counts": z["counts"].astype(np.uint32), "hits": z["hits"].astype(np.uint16),
+                "misses": z["misses"].astype(np.uint16), "sums": z["sums"].astype(np.float64).reshape(-1, 4)}
+
+
 def _align_out(twist, iterations, n_selected, rms, degenerate, converged):
     return np.array(twist, np.float32), {"iterations": int(iterations), "n_selected": int(n_selected),
                                          "rms": np.float32(rms), "degenerate": bool(degenerate),
@@ -1200,6 +1276,7 @@ class LaserMapping(_Handle):
     def enable_dense_map(self, leaf, max_voxels=DENSE_MAX_VOXELS):
         """Accumulate every mapped sweep's registered full-resolution cloud into a voxel map on the GPU (off by default)."""
         self._ck(self.L.loam_b200_map_dense_enable(self.h, np.float32(leaf), int(max_voxels)), "enableDenseMap")
+        self.dense_leaf = np.float32(leaf)
 
     def dense_stats(self):
         """{"voxels", "skipped", "dropped"} of the whole-run voxel map."""
@@ -1230,6 +1307,18 @@ class LaserMapping(_Handle):
         out = C.c_longlong(0)
         self._ck(self.L.loam_b200_map_debug_dense_table_slots(self.h, C.byref(out)), "denseTableSlots")
         return out.value
+
+    def dense_map_snapshot(self):
+        """BasicLaserMapping::denseMapSnapshot; returns what Ctx.dense_snapshot returns."""
+        return _dense_snapshot(lambda *a: self.L.loam_b200_map_dense_snapshot(self.h, *a), self.dense_stats()["voxels"],
+                               getattr(self, "dense_leaf", None), lambda rc: self._ck(rc, "denseMapSnapshot"))
+
+    def merge_dense_map(self, snap, twist6=None):
+        """BasicLaserMapping::mergeDenseMap; as Ctx.dense_merge."""
+        a = _merge_arrays(snap)
+        t = np.ascontiguousarray(twist6, np.float32).reshape(6) if twist6 is not None else None
+        self._ck(self.L.loam_b200_map_dense_merge(self.h, *_merge_ptrs(a), _fp(t) if t is not None else None),
+                 "mergeDenseMap")
 
     def build_dense_target(self, max_miss_ratio=None, radius=1, viewpoint=(0.0, 0.0, 0.0)):
         """BasicLaserMapping::buildDenseTarget: snapshot dense_map_normals(...) as the alignment target -> voxels."""

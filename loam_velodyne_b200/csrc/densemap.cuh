@@ -317,6 +317,136 @@ __global__ void dense_centroid_kernel(const DenseSlot* __restrict__ t, const int
   if (evidence) evidence[i] = e.evidence;
 }
 
+// ---- snapshots and merging (include/loam_b200.h "Whole-run voxel map snapshots and merging")
+// snapshot: the raw slot fields of the m compacted voxels in the sort's (ascending key) order
+__global__ void dense_snapshot_kernel(const DenseSlot* __restrict__ t, const int* __restrict__ slots,
+                                      const int* __restrict__ order, int m, unsigned long long* __restrict__ keys,
+                                      unsigned* __restrict__ counts, unsigned* __restrict__ evidence,
+                                      double4* __restrict__ sums) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const DenseSlot& e = t[slots[order[i]]];
+  keys[i] = e.key;
+  counts[i] = e.count;
+  evidence[i] = e.evidence;
+  sums[i] = make_double4(e.sum[0], e.sum[1], e.sum[2], e.sum[3]);
+}
+
+// rotation and translation of a merge, by value in the kernel arguments (on == 0: the sums are taken as they are)
+struct DenseMergePose {
+  double cx, sx, cy, sy, cz, sz;  // std::cos / std::sin of the pose's float rot_x, rot_y, rot_z (host)
+  double px, py, pz;              // the pose's float pos
+  int on;
+};
+
+// merge, one thread per entry, fp64 without FMA: S' = rotZ, rotX, rotY of (Sx, Sy, Sz) (dense_raycast's order) +
+// count * pos per axis, intensity unchanged (in place); the destination key is that of the fp32 centroid
+// (float)(S' / count) by the map's rule, DENSE_EMPTY when it is not finite or outside the key range.  Also the
+// (low word, index) pairs of the first sort pass.
+__global__ void dense_merge_key_kernel(double4* __restrict__ sums, const unsigned* __restrict__ counts, int n,
+                                       DenseMergePose a, float inv, unsigned long long* __restrict__ keys64,
+                                       unsigned* __restrict__ keys_lo, int* __restrict__ vals) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double4 s = sums[i];
+  const double c = (double)counts[i];
+  if (a.on) {
+    const double x1 = a.cz * s.x - a.sz * s.y, y1 = a.sz * s.x + a.cz * s.y;
+    const double y2 = a.cx * y1 - a.sx * s.z, z2 = a.sx * y1 + a.cx * s.z;
+    s.x = (a.cy * x1 + a.sy * z2) + c * a.px;
+    s.y = y2 + c * a.py;
+    s.z = (a.cy * z2 - a.sy * x1) + c * a.pz;
+    sums[i] = s;
+  }
+  const unsigned long long k =
+      dense_key_of(make_float4((float)(s.x / c), (float)(s.y / c), (float)(s.z / c), 0.f), inv);
+  keys64[i] = k;
+  keys_lo[i] = (unsigned)k;
+  vals[i] = i;
+}
+
+__device__ __forceinline__ unsigned dense_add_evidence(unsigned a, unsigned b) {
+  const unsigned h = (a & 0xffffu) + (b & 0xffffu), m = (a >> 16) + (b >> 16);
+  return (h < 0xffffu ? h : 0xffffu) | ((m < 0xffffu ? m : 0xffffu) << 16);
+}
+
+// merge, one thread per run head (sorted position i) -- dense_run_kernel over entries: the group's sums
+// ((0.0 + S'_1) + S'_2) + ... in ascending input index, counts added in uint32, hits and misses each added with
+// saturation; then the voxel's slot if the table already holds it.  The skipped entries (key DENSE_EMPTY, the last run)
+// add their counts to ctr->skipped.
+__global__ void dense_merge_run_kernel(const double4* __restrict__ sums, const unsigned* __restrict__ counts,
+                                       const unsigned* __restrict__ evidence, const unsigned long long* __restrict__ skey,
+                                       const int* __restrict__ order, const unsigned* __restrict__ pos,
+                                       const unsigned* __restrict__ block_off, int n, const DenseSlot* __restrict__ table,
+                                       unsigned long long mask, DenseRuns runs, unsigned* __restrict__ run_ev,
+                                       DenseCounters* __restrict__ ctr) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned pv = pos[i];
+  if (!(pv >> 31)) return;
+  const unsigned r = (pv & 0x7fffffffu) + block_off[i / SCAN_BS];
+  const unsigned long long k = skey[i];
+  double sx = 0.0, sy = 0.0, sz = 0.0, si = 0.0;
+  unsigned long long cnt = 0;
+  unsigned ev = 0;
+  for (int u = i; u < n && skey[u] == k; u++) {
+    const int o = order[u];
+    const double4 s = sums[o];
+    sx += s.x;
+    sy += s.y;
+    sz += s.z;
+    si += s.w;
+    cnt += counts[o];
+    ev = dense_add_evidence(ev, evidence[o]);
+  }
+  runs.key[r] = k;
+  runs.count[r] = (unsigned)cnt;
+  if (k == DENSE_EMPTY) {
+    runs.slot[r] = -2;
+    ctr->skipped += cnt;
+    return;
+  }
+  runs.sum[r] = make_double4(sx, sy, sz, si);
+  run_ev[r] = ev;
+  runs.slot[r] = dense_find(table, mask, k);
+}
+
+// merge -- dense_insert_kernel with the evidence of the runs instead of one hit per insert
+__global__ void dense_merge_insert_kernel(DenseRuns runs, const unsigned* __restrict__ run_ev,
+                                          const int* __restrict__ n_runs, const unsigned* __restrict__ rank,
+                                          const unsigned* __restrict__ block_off, DenseSlot* table,
+                                          unsigned long long mask, DenseCounters* __restrict__ ctr,
+                                          unsigned long long max_voxels) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= *n_runs) return;
+  const long long s = runs.slot[r];
+  if (s == -2) return;
+  const double4 p = runs.sum[r];
+  const unsigned cnt = runs.count[r];
+  if (s >= 0) {
+    DenseSlot& e = table[s];
+    e.count += cnt;
+    e.evidence = dense_add_evidence(e.evidence, run_ev[r]);
+    e.sum[0] += p.x;
+    e.sum[1] += p.y;
+    e.sum[2] += p.z;
+    e.sum[3] += p.w;
+    return;
+  }
+  const unsigned long long nr = rank[r] + block_off[r / SCAN_BS];
+  if (ctr->voxels + nr >= max_voxels) {
+    atomicAdd(&ctr->dropped, (unsigned long long)cnt);
+    return;
+  }
+  DenseSlot& e = table[dense_claim(table, mask, runs.key[r])];
+  e.count = cnt;
+  e.evidence = run_ev[r];
+  e.sum[0] = p.x;
+  e.sum[1] = p.y;
+  e.sum[2] = p.z;
+  e.sum[3] = p.w;
+}
+
 // ---- normals of the exported cloud (include/loam_b200.h "loam_b200_dense_export_normals")
 // first position in [lo, hi) of the ascending keys whose key is >= `key`
 __device__ __forceinline__ int dense_lower_bound(const unsigned long long* __restrict__ k, int lo, int hi,
@@ -1394,6 +1524,9 @@ struct DenseMap {
   DevBuf<float4> out;
   DevBuf<unsigned> out_count, out_evidence;
   DevBuf<float4> normals;         // export with normals: (nx, ny, nz, curvature) per exported voxel
+  DevBuf<double4> xsum;           // snapshot / merge: the entries' sums, counts and packed evidence (merge: in input
+  DevBuf<unsigned> xcount, xev;   // order, the sums transformed in place), and the evidence of the merge's runs
+  DevBuf<unsigned> run_ev;
   double vis_h_res = 0.0, vis_v_res = 0.0, vis_margin = 0.0;  // visibility pass (vis_h_res == 0: off)
   int vis_rows = 0, vis_cols = 0;
   DevBuf<unsigned> image;         // range image of the sweep being observed (float bits, DENSE_NO_RETURN when empty)
@@ -1432,6 +1565,7 @@ struct DenseMap {
     keys64.release(); skeys.release(); pos.release(); rank.release(); run_key.release(); run_count.release();
     run_sum.release(); run_slot.release(); slots.release(); ints.release(); out.release(); out_count.release();
     out_evidence.release(); normals.release(); image.release();
+    xsum.release(); xcount.release(); xev.release(); run_ev.release();
     ctr.release(); ctr_host.release();
     if (ev_in) cudaEventDestroy(ev_in);
     if (ev_done) cudaEventDestroy(ev_done);

@@ -94,6 +94,7 @@ void BasicLaserMapping::retainFromMapClouds(bool on) {
 
 void BasicLaserMapping::enableDenseMap(float leaf, long long maxVoxels) {
   _gpu->check(loam_b200_dense_enable(_gpu->get(), leaf, maxVoxels), "loam_b200_dense_enable");
+  _denseLeaf = leaf;
 }
 
 BasicLaserMapping::DenseMapStats BasicLaserMapping::denseMapStats() {
@@ -397,6 +398,36 @@ long long BasicLaserMapping::denseTableSlots() {
   long long n = 0;
   _gpu->check(loam_b200_debug_dense_table_slots(_gpu->get(), &n), "loam_b200_debug_dense_table_slots");
   return n;
+}
+
+void BasicLaserMapping::denseMapSnapshot(DenseMapSnapshot& out) {
+  const int n = (int)denseMapStats().voxels;
+  out.leaf = _denseLeaf;
+  out.keys.resize((size_t)n + 1);
+  out.counts.resize((size_t)n + 1);
+  out.hits.resize((size_t)n + 1);
+  out.misses.resize((size_t)n + 1);
+  out.sums.resize(4 * ((size_t)n + 1));
+  int got = 0;
+  _gpu->check(loam_b200_dense_snapshot(_gpu->get(), out.keys.data(), out.counts.data(), out.hits.data(),
+                                       out.misses.data(), out.sums.data(), n, &got),
+              "loam_b200_dense_snapshot");
+  out.keys.resize((size_t)got);
+  out.counts.resize((size_t)got);
+  out.hits.resize((size_t)got);
+  out.misses.resize((size_t)got);
+  out.sums.resize(4 * (size_t)got);
+}
+
+void BasicLaserMapping::mergeDenseMap(const DenseMapSnapshot& snap, const Twist* pose) {
+  const size_t n = snap.counts.size();
+  if (snap.hits.size() != n || snap.misses.size() != n || snap.sums.size() != 4 * n)
+    throw std::invalid_argument("BasicLaserMapping::mergeDenseMap: the snapshot's arrays differ in length");
+  loam_b200_pose p;
+  if (pose) b200::fillPose(*pose, p);
+  _gpu->check(loam_b200_dense_merge(_gpu->get(), snap.counts.data(), snap.hits.data(), snap.misses.data(),
+                                    snap.sums.data(), (int)n, pose ? &p : nullptr),
+              "loam_b200_dense_merge");
 }
 
 void BasicLaserMapping::clearDenseMap() {

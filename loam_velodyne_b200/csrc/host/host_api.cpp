@@ -542,6 +542,49 @@ int loam_b200_map_dense_export_normals(void* h, double max_miss_ratio, int radiu
     return 0;
   });
 }
+int loam_b200_map_dense_snapshot(void* h, unsigned long long* keys, unsigned int* counts, unsigned short* hits,
+                                 unsigned short* misses, double* sums, int cap, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (!n_out || cap < 0) { g_err = "loam_b200_map_dense_snapshot: bad capacity or NULL n_out"; return (int)LOAM_B200_ERR_ARG; }
+  return guarded([&] {
+    loam::BasicLaserMapping::DenseMapSnapshot s;
+    ((MapH*)h)->m.denseMapSnapshot(s);
+    const int n = (int)s.counts.size();
+    *n_out = n;
+    if (n > cap) { g_err = "loam_b200_map_dense_snapshot: output capacity too small"; return (int)LOAM_B200_ERR_CAPACITY; }
+    if (n == 0) return 0;
+    if (!counts || !sums) { g_err = "loam_b200_map_dense_snapshot: counts or sums is NULL"; return (int)LOAM_B200_ERR_ARG; }
+    if (keys) std::memcpy(keys, s.keys.data(), (size_t)n * sizeof(uint64_t));
+    std::memcpy(counts, s.counts.data(), (size_t)n * sizeof(uint32_t));
+    if (hits) std::memcpy(hits, s.hits.data(), (size_t)n * sizeof(uint16_t));
+    if (misses) std::memcpy(misses, s.misses.data(), (size_t)n * sizeof(uint16_t));
+    std::memcpy(sums, s.sums.data(), (size_t)n * 4 * sizeof(double));
+    return 0;
+  });
+}
+static std::vector<loam::Twist> twists_of(const float* t6, int k);
+int loam_b200_map_dense_merge(void* h, const unsigned int* counts, const unsigned short* hits,
+                              const unsigned short* misses, const double* sums, int n, const float* pose6) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && (!counts || !hits || !misses || !sums))) {
+    g_err = "loam_b200_map_dense_merge: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    loam::BasicLaserMapping::DenseMapSnapshot s;
+    s.counts.assign(counts, counts + n);
+    s.hits.assign(hits, hits + n);
+    s.misses.assign(misses, misses + n);
+    s.sums.assign(sums, sums + 4 * (size_t)n);
+    if (pose6) {
+      const loam::Twist t = twists_of(pose6, 1)[0];
+      ((MapH*)h)->m.mergeDenseMap(s, &t);
+    } else {
+      ((MapH*)h)->m.mergeDenseMap(s, nullptr);
+    }
+    return 0;
+  });
+}
 int loam_b200_map_dense_target_build(void* h, double max_miss_ratio, int radius, const double* viewpoint, int* n_out) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;
   if (!viewpoint || !n_out) { g_err = "loam_b200_map_dense_target_build: NULL argument"; return (int)LOAM_B200_ERR_ARG; }

@@ -146,6 +146,22 @@ class BasicLaserMapping {
                        const double viewpoint[3], std::vector<uint32_t>* counts = nullptr);
   /** Test hook (not in the reference): slots of the whole-run map's hash table (0 while the map is off). */
   long long denseTableSlots();
+  // Snapshots and merging of the whole-run map (include/loam_b200.h "Whole-run voxel map snapshots and merging"):
+  // denseMapSnapshot gives every stored voxel's exact state in ascending key order (sums: x, y, z, intensity per voxel,
+  // fp64); mergeDenseMap adds a snapshot into this map, as stored (pose nullptr) or under a rigid transform (e.g. the
+  // pose of another session's first sweep found by relocalizeInDenseTarget).  Each entry's voxel follows from its
+  // centroid at this map's leaf, so a snapshot of a finer map merges into a coarser one.  Resume a stopped run by
+  // merging its snapshot into an empty map of the same leaf: the result is the snapshot bit for bit.  Throws on a
+  // refused call (an entry with count 0 or hits 0, a sum or pose that is not finite, no dense map).
+  struct DenseMapSnapshot {
+    float leaf = 0.f;
+    std::vector<uint64_t> keys;
+    std::vector<uint32_t> counts;
+    std::vector<uint16_t> hits, misses;
+    std::vector<double> sums;  // 4 per voxel
+  };
+  void denseMapSnapshot(DenseMapSnapshot& out);
+  void mergeDenseMap(const DenseMapSnapshot& snap, const Twist* pose = nullptr);
   // Alignment against the whole-run map (include/loam_b200.h "Alignment against the whole-run voxel map"): point-to-plane
   // Gauss-Newton of a sensor-frame cloud against a target of voxel centroids and normals on the GPU -- relocalisation
   // in a map built earlier, drift checks of a mapped pose, another sensor's or session's sweeps in the same map.
@@ -289,6 +305,7 @@ class BasicLaserMapping {
   pcl::VoxelGrid<pcl::PointXYZI> _downSizeFilterCorner, _downSizeFilterSurf, _downSizeFilterMap;
   bool _downsizedMapCreated = false;
   bool _retainFromMap = false;
+  float _denseLeaf = 0.f;  // leaf of the whole-run map (0 = never enabled)
   bool _sharded = false;
   int _shardRank = 0, _shardWorld = 1, _shardSlab = 0;  // cube-sharded map (0 = off)
 

@@ -815,6 +815,65 @@ int loam_b200_dense_relocalize_global(loam_b200_ctx* ctx, const float* xyzi, int
 int loam_b200_debug_dense_place_descriptors(loam_b200_ctx* ctx, float* out, long long cap, long long* n_out);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Euclidean segmentation of the whole-run voxel map and of clouds (csrc/densemap.cuh, DESIGN.md "Euclidean
+ * segmentation"): which voxels or points belong together -- dropping small specks from an export, grouping the points
+ * of a sweep that the map does not explain into objects.  pcl::EuclideanClusterExtraction's semantics, computed exactly.
+ * Not on the per-sweep path; neither call changes the map, the target or any product of the target (ray index,
+ * distance field, place database).
+ *   entries: each has a float position p_i and a key k_i of the map's codec at cell size `cell`.
+ *     dense_segment: the target's voxels in ascending key order (dense_raycast's index), p_i = the centroid, k_i = the
+ *       target's key, cell = the target's leaf.  A built or a loaded target.
+ *     cloud_segment: n points (float[4], w ignored; host memory, or device memory when on_device != 0); k_i =
+ *       floorf(c * (1.0f / tol)) per axis as the map keys a point (cell = tol).  A point that is not finite or whose
+ *       voxel lies outside [-2^20, 2^20) is not an entry (label -1), as the insertion skips it.
+ *   candidates: r = floor((double)tol / (double)cell) + 1; the pairs (i, j) whose voxels lie within r voxels of each
+ *     other on every axis (the rows of dense_box_walk: per (z, y) row inside the key range, never wrapping).  Two
+ *     points within tol lie at most ceil(tol / cell) <= r cells apart on each axis in exact arithmetic.  The keying is
+ *     monotonic, and fp32 keying or a centroid's fp32 rounding moves a point across at most the one face it lies on;
+ *     where tol / cell is an integer (always in cloud mode) the +1 leaves the spare cell that absorbs that move, and
+ *     elsewhere the pair would have to lie further than tol apart to gain a cell.  Only a tol / cell within a few
+ *     fp32 ulps below an integer leaves a pair at the very limit outside; the box at r is the definition.
+ *   edge: a candidate pair with d2 <= (double)tol * (double)tol, d2 = (dx*dx + dy*dy) + dz*dz, dx = (double)p_i.x -
+ *     (double)p_j.x (likewise y, z), fp64 without FMA, each operation rounded on its own.
+ *   segment: a connected component of the edge graph; those with min_size <= size <= max_size are kept.
+ *   rank: size descending, ties by the smallest entry index (the position in key order for a target, the input index
+ *     for a cloud); ids 0..K-1 in that order.
+ *   labels[i]: the entry's segment id, -1 when its segment was filtered out or it is not an entry; in entry order (key
+ *     order for a target, input order for a cloud).  May be NULL.
+ *   record: size, first = the smallest entry index, lo / hi = the float min / max of the members' coordinates per axis,
+ *     centroid = (float)(sum / size) per axis.  The fp64 sums: members in ascending entry index, in consecutive chunks
+ *     of 256 from the segment's first member; each chunk summed one member after the other from 0.0 ((double) of the
+ *     float coordinate), then the chunk sums added in chunk order from 0.0.
+ *   out: segments[0 .. K) and *n_out = K; LOAM_B200_ERR_CAPACITY (with *n_out = K, nothing else written) when K > cap.
+ * Union-find with atomic hooks of the larger root under the smaller: every root is the smallest member of its
+ * component, so the result does not depend on thread scheduling; every output above is exact and reproducible.
+ * LOAM_B200_ERR_ARG: tol not finite or not > 0, tol / leaf > 4 for a target (r <= 5, at most 121 rows per entry; for a
+ * coarser tolerance merge a snapshot into a coarser map and build a target from it), min_size < 1, min_size >
+ * max_size, n < 0, cap < 0, a NULL pointer (segments with cap > 0, n_out; xyzi with n > 0).  dense_segment without a
+ * target: LOAM_B200_ERR_STATE.  Every check runs on the host before anything is launched, so a refused call changes
+ * nothing.  An empty target or cloud launches nothing (K = 0).  Synchronous.  Launches count under LOAM_B200_K_DENSE,
+ * a fixed number per call for a given entry count (the union-find runs one pass, whatever the data).
+ * Cost: the union pass visits, per entry, every entry of its box of (2r + 1)^3 voxels.  A target holds one entry per
+ * voxel and r <= 5, so that is at most 1331 visits per entry.  A cloud is keyed at cell = tol, so one voxel holds every
+ * point of a tol-sized cube and the pass grows with the square of the points per voxel: O(n^2) when a whole cloud
+ * falls into a few voxels (a tolerance of metres on a dense sweep, most of whose points lie near the sensor).  For a
+ * large tolerance, thin the cloud first (loam_b200_voxel_grid at a fraction of tol) or segment a target built from it.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t size;        /* members */
+  int32_t first;       /* the smallest entry index of its members */
+  float lo[3], hi[3];  /* min / max of the members' x, y, z */
+  float centroid[3];   /* (float)(fp64 sum / size) per axis */
+} loam_b200_segment;
+
+/* the current target's voxels: the length of dense_segment's labels (LOAM_B200_ERR_STATE without a target) */
+int loam_b200_dense_target_size(loam_b200_ctx* ctx, int* n_out);
+int loam_b200_dense_segment(loam_b200_ctx* ctx, float tol, int min_size, int max_size, int32_t* labels,
+                            loam_b200_segment* segments, int cap, int* n_out);
+int loam_b200_cloud_segment(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device, float tol, int min_size,
+                            int max_size, int32_t* labels, loam_b200_segment* segments, int cap, int* n_out);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice
  * of the corner and surface queries; with a communicator the 32-float partial normal equations are all-reduced
  * (NCCL, sum, fp32) on the context's stream directly behind the kernel, so every rank returns the same totals and

@@ -170,6 +170,13 @@ int loam_b200_map_dense_relocalize_global(void* h, const float* xyzi, int n, int
                                           int yaw_steps, float xz_step, int xz_steps,
                                           const loam_b200_reloc_params* prm, loam_b200_reloc_candidate* out, int cap,
                                           int* n_out);
+/* Euclidean segmentation of that target (BasicLaserMapping::segmentDenseTarget, include/loam_b200.h "Euclidean
+ * segmentation of the whole-run voxel map and of clouds"), same in-flight rule: labels (may be NULL) receive one int
+ * per target voxel, as many as loam_b200_map_dense_target_size (BasicLaserMapping::denseTargetSize) reports;
+ * segments[0 .. *n_out), LOAM_B200_ERR_CAPACITY when *n_out > cap. */
+int loam_b200_map_dense_target_size(void* h, int* n_out);
+int loam_b200_map_dense_segment(void* h, float tol, int min_size, int max_size, int* labels,
+                                loam_b200_segment* segments, int cap, int* n_out);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank
  * then enables sharding on its mapping object (nccl_id128 = NULL: slice the queries only, no collective) */
 int loam_b200_host_nccl_unique_id(unsigned char* out128);

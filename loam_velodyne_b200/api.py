@@ -105,6 +105,16 @@ PLACE_SPACING, PLACE_TOP_M = 4.0, 5
 PLACE_YAW_STEP_DEG, PLACE_YAW_STEPS, PLACE_XZ_STEP, PLACE_XZ_STEPS = 2.0, 3, 0.4, 5
 
 
+# loam_b200_segment as a numpy record (the segment array of dense_segment / segment_cloud is filled in place)
+SEGMENT_DTYPE = np.dtype([("size", "<i4"), ("first", "<i4"), ("lo", "<f4", 3), ("hi", "<f4", 3),
+                          ("centroid", "<f4", 3)])
+
+
+class Segment(C.Structure):
+    _fields_ = [("size", C.c_int32), ("first", C.c_int32), ("lo", C.c_float * 3), ("hi", C.c_float * 3),
+                ("centroid", C.c_float * 3)]
+
+
 class NormalEq(C.Structure):
     _fields_ = [("AtA", C.c_float * 36), ("AtB", C.c_float * 6), ("n_selected", C.c_int),
                 ("n_corner_selected", C.c_int)]
@@ -245,6 +255,10 @@ def lib():
                                                         C.c_float, C.c_int, C.POINTER(RelocParams),
                                                         C.POINTER(RelocCandidate), C.c_int, _I]),
         "loam_b200_debug_dense_place_descriptors": (C.c_int, [vp, _F, C.c_longlong, _LL]),
+        "loam_b200_dense_target_size": (C.c_int, [vp, _I]),
+        "loam_b200_dense_segment": (C.c_int, [vp, C.c_float, C.c_int, C.c_int, _I, C.POINTER(Segment), C.c_int, _I]),
+        "loam_b200_cloud_segment": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _I,
+                                              C.POINTER(Segment), C.c_int, _I]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -315,6 +329,9 @@ def lib():
         "loam_b200_map_dense_relocalize_global": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_float, C.c_int, C.c_float,
                                                             C.c_int, C.POINTER(RelocParams),
                                                             C.POINTER(RelocCandidate), C.c_int, _I]),
+        "loam_b200_map_dense_target_size": (C.c_int, [vp, _I]),
+        "loam_b200_map_dense_segment": (C.c_int, [vp, C.c_float, C.c_int, C.c_int, _I, C.POINTER(Segment), C.c_int,
+                                                  _I]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_map_kernel_profile": (C.c_int, [vp, C.c_int, _D]),
@@ -909,6 +926,32 @@ class Ctx:
         self._ck(self.L.loam_b200_debug_dense_distance_bytes(self.h, C.byref(out)), "dense_distance_bytes")
         return out.value
 
+    # ---- Euclidean segmentation (include/loam_b200.h "Euclidean segmentation of the whole-run voxel map and of clouds")
+    def dense_segment(self, tolerance, min_size=1, max_size=None):
+        """Euclidean segments of the target's voxels (centroids within tolerance metres, at most 4 leaves) with
+        min_size <= size <= max_size -> (labels int32[N]: per target voxel in key order, its segment's rank or -1;
+        segments: dict of arrays size, first, lo, hi, centroid), ranked by size descending, ties by first."""
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_target_size(self.h, C.byref(n)), "dense_segment")
+        return _segment_call(lambda lab, seg, cap, k: self.L.loam_b200_dense_segment(
+            self.h, np.float32(tolerance), int(min_size), _max_size(max_size), lab, seg, cap, k), n.value,
+            lambda rc: self._ck(rc, "dense_segment"))
+
+    def dense_target_size(self):
+        """Voxels of the current target (the length of dense_segment's labels); raises without a target."""
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_target_size(self.h, C.byref(n)), "dense_target_size")
+        return n.value
+
+    def segment_cloud(self, pts, tolerance, min_size=1, max_size=None, on_device=False, n=None):
+        """Euclidean segments of a cloud's points (N x 4, w ignored; with on_device=True the address of n float[4] in
+        device memory); needs no map and no target -> (labels int32[N] in input order, -1 for points not kept or not
+        finite; segments as dense_segment, first = the smallest input index)."""
+        ptr, k = _pts_or_device(pts, on_device, n)
+        return _segment_call(lambda lab, seg, cap, kk: self.L.loam_b200_cloud_segment(
+            self.h, ptr, k, 1 if on_device else 0, np.float32(tolerance), int(min_size), _max_size(max_size), lab,
+            seg, cap, kk), k, lambda rc: self._ck(rc, "segment_cloud"))
+
     # ---- place recognition (include/loam_b200.h "Place recognition and global relocalisation")
     def place_descriptor(self, pts, params=None, on_device=False, n=None):
         """Polar height descriptor of sensor-frame pts (N x 4, w ignored) -> float32 (rings, sectors).  With
@@ -1105,6 +1148,20 @@ def _pts_or_device(pts, on_device, n):
         return C.cast(C.c_void_p(int(pts)), _F), int(n)
     a = _pts(pts)
     return _fp(a), a.shape[0]
+
+
+def _max_size(max_size):
+    return 2147483647 if max_size is None else int(max_size)
+
+
+def _segment_call(call, n, ck):
+    """call(labels, segments, cap, n_out) with room for n entries (K <= n) -> (labels int32[n], dict of the K
+    segments' fields)."""
+    labels = np.zeros(max(n, 1), np.int32)
+    seg = np.zeros(max(n, 1), SEGMENT_DTYPE)
+    k = C.c_int(0)
+    ck(call(_ip(labels), seg.ctypes.data_as(C.POINTER(Segment)), n, C.byref(k)))
+    return labels[:n].copy(), {f: seg[f][:k.value].copy() for f in SEGMENT_DTYPE.names}
 
 
 def _box_args(lo, dims):
@@ -1395,6 +1452,14 @@ class LaserMapping(_Handle):
         self._ck(self.L.loam_b200_map_dense_raycast(self.h, _fp(a), k, _fp(t), np.float32(min_range),
                                                     np.float32(max_range), _fp(rng), _ip(idx)), "raycastDenseTarget")
         return rng[:k].copy(), idx[:k].copy()
+
+    def segment_dense_target(self, tolerance, min_size=1, max_size=None):
+        """BasicLaserMapping::segmentDenseTarget; returns what Ctx.dense_segment returns."""
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_map_dense_target_size(self.h, C.byref(n)), "segmentDenseTarget")
+        return _segment_call(lambda lab, seg, cap, k: self.L.loam_b200_map_dense_segment(
+            self.h, np.float32(tolerance), int(min_size), _max_size(max_size), lab, seg, cap, k), n.value,
+            lambda rc: self._ck(rc, "segmentDenseTarget"))
 
     def build_dense_distance_field(self, lo, dims, max_distance, download=True):
         """BasicLaserMapping::buildDenseDistanceField; as Ctx.dense_distance_field."""

@@ -186,6 +186,7 @@ struct SortScratch {
 
 struct DenseMap;  // whole-run voxel map (densemap.cuh), created by loam_b200_dense_enable
 struct DenseTarget;  // registration target of loam_b200_dense_align (densemap.cuh)
+struct DenseSegScratch;  // scratch of loam_b200_cloud_segment (densemap.cuh)
 
 }  // namespace loamb
 
@@ -371,6 +372,8 @@ struct loam_b200_ctx {
   loamb::DenseMap* dense = nullptr;
   // its registration target: null until the first loam_b200_dense_target_build / _load succeeds
   loamb::DenseTarget* target = nullptr;
+  // scratch of the cloud segmentation: null until the first loam_b200_cloud_segment with points
+  loamb::DenseSegScratch* seg = nullptr;
 };
 
 namespace loamb {

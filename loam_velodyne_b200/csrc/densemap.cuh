@@ -1502,6 +1502,240 @@ dense_carve_kernel(const float4* __restrict__ p, int n, DenseCarveArgs a, DenseB
   }
 }
 
+// ---- Euclidean segmentation (include/loam_b200.h "Euclidean segmentation of the whole-run voxel map and of clouds")
+// Entries: sorted keys skey[0, n) (a cloud's skipped points carry DENSE_EMPTY and sort last) and their positions spos
+// in the same order; orig / inv (cloud mode) map sorted position <-> input index, null for a target (identity).  The
+// entry index e of sorted position i is orig[i] (cloud) or i (target).
+// Union-find over sorted positions (ECL-CC): par[x] <= x always, because a hook puts the larger root under the
+// smaller one and path halving only moves a pointer to an ancestor.  So every non-root points to a smaller index and
+// the root of a tree is its smallest member: the final roots -- and every label and record derived from them -- are a
+// function of the edge set alone, whatever order the threads hook in.  The bit-for-bit tests rely on this.
+constexpr int DENSE_SEG_CHUNK = 256;             // members per chunk of the fixed-order fp64 sums
+constexpr unsigned DENSE_SEG_NONE = 0xffffffffu;  // sort key of an entry outside every kept segment (sorts last)
+
+// root of x with path halving (L2 loads: other SMs hook concurrently; a stale parent only costs a retry)
+__device__ __forceinline__ int dense_seg_find(int* par, int x) {
+  int cur = __ldcg(&par[x]);
+  if (cur == x) return x;
+  int prev = x, next;
+  while (cur > (next = __ldcg(&par[cur]))) {
+    __stcg(&par[prev], next);
+    prev = cur;
+    cur = next;
+  }
+  return cur;
+}
+
+// join the components of a and b: hook the larger root under the smaller with atomicCAS; a failed CAS returns the
+// node's new parent (smaller), from which the next attempt climbs
+__device__ __forceinline__ void dense_seg_unite(int* par, int a, int b) {
+  int ra = dense_seg_find(par, a), rb = dense_seg_find(par, b);
+  while (ra != rb) {
+    if (ra > rb) {
+      const int t = ra;
+      ra = rb;
+      rb = t;
+    }
+    const int old = atomicCAS(&par[rb], rb, ra);
+    if (old == rb) return;
+    rb = old;
+  }
+}
+
+// cloud mode: key, position and index maps in sorted order (order: the stable two-pass key sort)
+__global__ void dense_seg_gather_kernel(const unsigned long long* __restrict__ keys64, const int* __restrict__ order,
+                                        int n, const float4* __restrict__ p, unsigned long long* __restrict__ skey,
+                                        float4* __restrict__ spos, int* __restrict__ orig, int* __restrict__ inv) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int o = order[i];
+  skey[i] = keys64[o];
+  spos[i] = p[o];
+  orig[i] = o;
+  inv[o] = i;
+}
+
+__global__ void dense_seg_init_kernel(int n, int* __restrict__ par, int* __restrict__ size, int* __restrict__ first,
+                                      int* __restrict__ segid) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  par[i] = i;
+  size[i] = 0;
+  first[i] = 0x7fffffff;
+  segid[i] = -1;
+}
+
+// One thread per entry: the entries j > i of dense_box_walk at `radius` with d2 = (dx*dx + dy*dy) + dz*dz <= tol2,
+// fp64 of the float coordinates without FMA, join i's component.
+__global__ void __launch_bounds__(128)
+dense_seg_union_kernel(const unsigned long long* __restrict__ skey, const float4* __restrict__ spos, int n, int radius,
+                       double tol2, int* par) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long key = skey[i];
+  if (key == DENSE_EMPTY) return;
+  const float4 pi = spos[i];
+  const double px = (double)pi.x, py = (double)pi.y, pz = (double)pi.z;
+  dense_box_walk(skey, n, key, radius, [&](int j) {
+    if (j <= i) return;
+    const float4 pj = spos[j];
+    const double dx = px - (double)pj.x, dy = py - (double)pj.y, dz = pz - (double)pj.z;
+    if ((dx * dx + dy * dy) + dz * dz <= tol2) dense_seg_unite(par, i, j);
+  });
+}
+
+// flatten: every entry's root (-1: not an entry); sizes and smallest entry index accumulate on the roots
+__global__ void dense_seg_root_kernel(const unsigned long long* __restrict__ skey, int n, const int* __restrict__ orig,
+                                      int* par, int* __restrict__ root, int* __restrict__ size, int* __restrict__ first) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (skey[i] == DENSE_EMPTY) {
+    root[i] = -1;
+    return;
+  }
+  const int r = dense_seg_find(par, i);
+  root[i] = r;
+  atomicAdd(&size[r], 1);
+  atomicMin(&first[r], orig ? orig[i] : i);
+}
+
+// rank keys, one thread per entry index e: a kept root is written at its smallest entry index (keys_lo =
+// 0xffffffff - size, vals = root), everything else sorts last.  A stable sort of these 32-bit keys then ranks by size
+// descending, ties by smallest entry index ascending.  *kept counts the segments.
+__global__ void dense_seg_rank_key_kernel(int n, const int* __restrict__ inv, const int* __restrict__ root,
+                                          const int* __restrict__ size, const int* __restrict__ first, int min_size,
+                                          int max_size, unsigned* __restrict__ keys_lo, int* __restrict__ vals,
+                                          int* __restrict__ kept) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const int r = root[inv ? inv[e] : e];
+  unsigned k = DENSE_SEG_NONE;
+  if (r >= 0 && first[r] == e && size[r] >= min_size && size[r] <= max_size) {
+    k = 0xffffffffu - (unsigned)size[r];
+    atomicAdd(kept, 1);
+  }
+  keys_lo[e] = k;
+  vals[e] = r;
+}
+
+// ids in ranked order: segid[root] = rank, segroot[rank] = root
+__global__ void dense_seg_id_kernel(const unsigned* __restrict__ keys, const int* __restrict__ vals, int n,
+                                    int* __restrict__ segid, int* __restrict__ segroot) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n || keys[r] == DENSE_SEG_NONE) return;
+  segid[vals[r]] = r;
+  segroot[r] = vals[r];
+}
+
+// labels in entry order, and the member keys (segment id, in entry order; vals = sorted position) whose stable sort
+// groups each segment's members in ascending entry index
+__global__ void dense_seg_label_kernel(int n, const int* __restrict__ inv, const int* __restrict__ root,
+                                       const int* __restrict__ segid, int* __restrict__ labels,
+                                       unsigned* __restrict__ keys_lo, int* __restrict__ vals) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const int i = inv ? inv[e] : e;
+  const int r = root[i];
+  const int id = r < 0 ? -1 : segid[r];
+  labels[e] = id;
+  keys_lo[e] = id < 0 ? DENSE_SEG_NONE : (unsigned)id;
+  vals[e] = i;
+}
+
+// first member position of each segment in the grouped order
+__global__ void dense_seg_head_kernel(const unsigned* __restrict__ keys, int n, int* __restrict__ start) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const unsigned id = keys[p];
+  if (id != DENSE_SEG_NONE && (p == 0 || keys[p - 1] != id)) start[id] = p;
+}
+
+// min / max that keep the earlier value on a tie (strict <, >), so the sign of a zero is that of the first member
+// in entry order to reach the extreme
+__device__ __forceinline__ void dense_seg_extend(float4& lo, float4& hi, const float4& a, const float4& b) {
+  if (a.x < lo.x) lo.x = a.x;
+  if (a.y < lo.y) lo.y = a.y;
+  if (a.z < lo.z) lo.z = a.z;
+  if (b.x > hi.x) hi.x = b.x;
+  if (b.y > hi.y) hi.y = b.y;
+  if (b.z > hi.z) hi.z = b.z;
+}
+
+// one thread per chunk head (every DENSE_SEG_CHUNK-th member of a segment from its first): the chunk's members in
+// ascending entry index summed one after the other in fp64 from 0.0, and their float min / max
+__global__ void dense_seg_chunk_kernel(const unsigned* __restrict__ keys, const int* __restrict__ vals, int n,
+                                       const float4* __restrict__ spos, const int* __restrict__ start,
+                                       double4* __restrict__ csum, float4* __restrict__ clo, float4* __restrict__ chi) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const unsigned id = keys[p];
+  if (id == DENSE_SEG_NONE || (p - start[id]) % DENSE_SEG_CHUNK) return;
+  double sx = 0.0, sy = 0.0, sz = 0.0;
+  float4 lo = spos[vals[p]], hi = lo;
+  const int end = min(n, p + DENSE_SEG_CHUNK);
+  for (int u = p; u < end && keys[u] == id; u++) {
+    const float4 q = spos[vals[u]];
+    sx += (double)q.x;
+    sy += (double)q.y;
+    sz += (double)q.z;
+    dense_seg_extend(lo, hi, q, q);
+  }
+  csum[p] = make_double4(sx, sy, sz, 0.0);
+  clo[p] = lo;
+  chi[p] = hi;
+}
+
+// one thread per segment: the chunk sums added in chunk order from 0.0, min / max over the chunks, the record
+__global__ void dense_seg_record_kernel(const int* __restrict__ kept, const int* __restrict__ start,
+                                        const int* __restrict__ segroot, const int* __restrict__ size,
+                                        const int* __restrict__ first, const double4* __restrict__ csum,
+                                        const float4* __restrict__ clo, const float4* __restrict__ chi,
+                                        loam_b200_segment* __restrict__ out) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= *kept) return;
+  const int s = start[r], root = segroot[r], m = size[root];
+  double sx = 0.0, sy = 0.0, sz = 0.0;
+  float4 lo = clo[s], hi = chi[s];
+  for (int p = s; p < s + m; p += DENSE_SEG_CHUNK) {
+    const double4 q = csum[p];
+    sx += q.x;
+    sy += q.y;
+    sz += q.z;
+    dense_seg_extend(lo, hi, clo[p], chi[p]);
+  }
+  loam_b200_segment g;
+  g.size = m;
+  g.first = first[root];
+  g.lo[0] = lo.x;
+  g.lo[1] = lo.y;
+  g.lo[2] = lo.z;
+  g.hi[0] = hi.x;
+  g.hi[1] = hi.y;
+  g.hi[2] = hi.z;
+  const double c = (double)m;
+  g.centroid[0] = (float)(sx / c);
+  g.centroid[1] = (float)(sy / c);
+  g.centroid[2] = (float)(sz / c);
+  out[r] = g;
+}
+
+// Scratch of one segmentation: DenseTarget::seg for the target, loam_b200_ctx::seg for clouds; kept for the next call
+struct DenseSegScratch {
+  DevBuf<unsigned long long> keys64, skey;  // cloud: input keys, sorted keys
+  DevBuf<float4> pts, spos;                 // cloud: input points (host upload), sorted positions
+  DevBuf<int> orig, inv;                    // cloud: sorted position <-> input index
+  DevBuf<int> par, root, size, first, segid, segroot, start, labels, ints;
+  DevBuf<double4> csum;
+  DevBuf<float4> clo, chi;
+  DevBuf<loam_b200_segment> out;
+
+  void release() {
+    keys64.release(); skey.release(); pts.release(); spos.release(); orig.release(); inv.release(); par.release();
+    root.release(); size.release(); first.release(); segid.release(); segroot.release(); start.release();
+    labels.release(); ints.release(); csum.release(); clo.release(); chi.release(); out.release();
+  }
+};
+
 // Host-side state of the map (loam_b200_ctx::dense).  The insertion runs on its own stream with its own sort scratch,
 // so the next sweep's stages on the main stream and the map update on its lanes neither wait for it nor share buffers.
 struct DenseMap {
@@ -1617,6 +1851,7 @@ struct DenseTarget {
   DevBuf<float> dist_f;                 // the float distances of a build that downloads them
   DevBuf<int> edt_g, edt_b, edt_s, edt_t, edt_v;
   DevBuf<float> qdist, qgrad;
+  DenseSegScratch seg;                  // loam_b200_dense_segment
 
   void release() {
     keys.release(); keys64.release(); cent.release(); nrm.release(); pts.release(); args.release(); partials.release();
@@ -1629,6 +1864,7 @@ struct DenseTarget {
     place_k = 0;
     dist_sq.release(); dist_f.release(); edt_g.release(); edt_b.release(); edt_s.release(); edt_t.release();
     edt_v.release(); qdist.release(); qgrad.release();
+    seg.release();
     dist_ready = false;
     ray = DenseBrickIndex{};
     n = 0;

@@ -198,6 +198,38 @@ void BasicLaserMapping::loadDenseTarget(float leaf, const pcl::PointCloud<pcl::P
               "loam_b200_dense_target_load");
 }
 
+size_t BasicLaserMapping::denseTargetSize() {
+  int n = 0;
+  _gpu->check(loam_b200_dense_target_size(_gpu->get(), &n), "loam_b200_dense_target_size");
+  return (size_t)n;
+}
+
+std::vector<BasicLaserMapping::DenseSegment> BasicLaserMapping::segmentDenseTarget(float tolerance, int minSize,
+                                                                                   int maxSize,
+                                                                                   std::vector<int>* labels) {
+  const size_t n = denseTargetSize();  // the labels' length, and K <= n
+  std::vector<loam_b200_segment> seg(n + 1);
+  std::vector<int32_t> lab(labels ? n + 1 : 0);
+  int k = 0;
+  _gpu->check(loam_b200_dense_segment(_gpu->get(), tolerance, minSize, maxSize, labels ? lab.data() : nullptr,
+                                      seg.data(), (int)n, &k),
+              "loam_b200_dense_segment");
+  if (labels) labels->assign(lab.begin(), lab.begin() + (ptrdiff_t)n);
+  std::vector<DenseSegment> out((size_t)k);
+  for (int i = 0; i < k; i++) {
+    const loam_b200_segment& g = seg[(size_t)i];
+    DenseSegment& o = out[(size_t)i];
+    o.size = (size_t)g.size;
+    o.first = (size_t)g.first;
+    for (int a = 0; a < 3; a++) {
+      o.lo[a] = g.lo[a];
+      o.hi[a] = g.hi[a];
+      o.centroid[a] = g.centroid[a];
+    }
+  }
+  return out;
+}
+
 static Twist twistOf(const float rot[3], const float pos[3]) {
   Twist t;
   t.rot_x = rot[0];

@@ -786,6 +786,46 @@ int loam_b200_map_dense_distance_query(void* h, const float* xyzi, int n, float*
     return 0;
   });
 }
+int loam_b200_map_dense_target_size(void* h, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (!n_out) {
+    g_err = "loam_b200_map_dense_target_size: NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    *n_out = (int)((MapH*)h)->m.denseTargetSize();
+    return 0;
+  });
+}
+int loam_b200_map_dense_segment(void* h, float tol, int min_size, int max_size, int* labels,
+                                loam_b200_segment* segments, int cap, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (cap < 0 || (cap > 0 && !segments) || !n_out) {
+    g_err = "loam_b200_map_dense_segment: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    std::vector<int> lab;
+    const auto seg = m->m.segmentDenseTarget(tol, min_size, max_size, labels ? &lab : nullptr);
+    *n_out = (int)seg.size();
+    if ((int)seg.size() > cap) {
+      g_err = "loam_b200_map_dense_segment: output capacity too small";
+      return (int)LOAM_B200_ERR_CAPACITY;
+    }
+    for (size_t i = 0; i < seg.size(); i++) {
+      segments[i].size = (int32_t)seg[i].size;
+      segments[i].first = (int32_t)seg[i].first;
+      for (int a = 0; a < 3; a++) {
+        segments[i].lo[a] = seg[i].lo[a];
+        segments[i].hi[a] = seg[i].hi[a];
+        segments[i].centroid[a] = seg[i].centroid[a];
+      }
+    }
+    if (labels && !lab.empty()) std::memcpy(labels, lab.data(), lab.size() * sizeof(int));
+    return 0;
+  });
+}
 static loam::BasicLaserMapping::PlaceParams place_params_of(const loam_b200_place_params& p) {
   loam::BasicLaserMapping::PlaceParams o;
   o.rings = p.rings;

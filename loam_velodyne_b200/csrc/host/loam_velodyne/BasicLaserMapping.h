@@ -272,6 +272,22 @@ class BasicLaserMapping {
                                                             const GlobalGrid& grid = GlobalGrid(),
                                                             const RelocParams& params = RelocParams(),
                                                             size_t maxCandidates = 16);
+  // Euclidean segmentation of the target (include/loam_b200.h "Euclidean segmentation of the whole-run voxel map and
+  // of clouds"; pcl::EuclideanClusterExtraction over the target's voxels, exact): connected components of the voxels
+  // whose centroids lie within `tolerance` metres (at most 4 leaves), kept when their size is in [minSize, maxSize],
+  // ranked by size descending (ties: smallest voxel index first).  labels (optional): per target voxel, in the
+  // target's order (raycastDenseTarget's index), its segment's rank or -1.  Throws without a target and on bad
+  // arguments.
+  struct DenseSegment {
+    size_t size;         // voxels
+    size_t first;        // the smallest target index among them
+    float lo[3], hi[3];  // min / max of their centroids per axis
+    float centroid[3];   // mean of their centroids
+  };
+  // voxels of the current target (the length of segmentDenseTarget's labels); throws without a target
+  size_t denseTargetSize();
+  std::vector<DenseSegment> segmentDenseTarget(float tolerance, int minSize = 1, int maxSize = 2147483647,
+                                               std::vector<int>* labels = nullptr);
 
  private:
   typedef pcl::PointCloud<pcl::PointXYZI> Cloud;

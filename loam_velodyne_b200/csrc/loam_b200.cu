@@ -736,6 +736,11 @@ int loam_b200_destroy(loam_b200_ctx* c) {
     delete c->target;
     c->target = nullptr;
   }
+  if (c->seg) {
+    c->seg->release();
+    delete c->seg;
+    c->seg = nullptr;
+  }
   c->reg_pts.release(); c->reg_ring_start.release(); c->reg_ring_end.release(); c->reg_picks.release();
   c->reg_counts.release(); c->reg_label.release(); c->reg_lessflat.release(); c->stage.release(); c->stage2.release();
   for (auto& t : c->tree) {

@@ -874,6 +874,67 @@ int loam_b200_cloud_segment(loam_b200_ctx* ctx, const float* xyzi, int n, int on
                             int max_size, int32_t* labels, loam_b200_segment* segments, int cap, int* n_out);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Ground of the whole-run voxel map (csrc/densemap.cuh dense_ground_*, DESIGN.md "Ground patches"): which target
+ * voxels are ground, the segmentation of everything else, and which points of a sweep lie on the ground the map
+ * knows -- the step before grouping objects.  The map frame is LOAM's, y up: the ground plane is x-z.  Not on the
+ * per-sweep path; no call changes the map, the target, its ray index, distance field or place database, or an earlier
+ * segmentation's result.  Synchronous.  Launches count under LOAM_B200_K_DENSE.
+ * dense_ground (a built or loaded target; params below):
+ *   candidate: a target voxel whose normal_x is not NaN and (double)fabsf(n_y) >= cos_max, cos_max = cos(max_slope_deg
+ *     * pi / 180) in double (the normal's orientation is irrelevant), and n_w <= max_curvature in fp32 (a NaN w fails)
+ *     unless max_curvature is +inf, which skips the curvature test (a loaded target whose w means nothing).
+ *   candidate pairs: dense_box_walk at r = floor(max(tol, max_step) / leaf) + 1 over the candidates in key order.
+ *   edge: both candidates, dx*dx + dz*dz <= tol^2 and |dy| <= max_step, in fp64 of the float centroids without FMA,
+ *     each operation rounded on its own (tol^2 = (double)tol * (double)tol).  A horizontal distance with a step bound:
+ *     a ramp within the slope limit joins, a kerb up to max_step joins, a table top or a car roof does not.
+ *   patch: a connected component of the candidates with size >= min_size.  Rank, ids, records (loam_b200_segment),
+ *     the fp64 chunk sums and LOAM_B200_ERR_CAPACITY are dense_segment's, with the target index as the entry index
+ *     (first, ties).  labels[i] (may be NULL): per target voxel in key order, its patch id or -1.
+ *   product: the ground flags (a voxel is ground when it lies in a patch), stored with the target on LOAM_B200_OK and
+ *     on LOAM_B200_ERR_CAPACITY (capacity only limits the records written).  A later dense_ground replaces them; a
+ *     target build, load or release drops them, like the ray index, distance field and place database.
+ *   Limitation: a large flat upward surface with no step to the street, such as a rooftop, is a patch like the street;
+ *     its records' lo[1] / hi[1] let the caller reject it by height.
+ *   LOAM_B200_ERR_ARG: tol or max_step not finite and > 0, max(tol, max_step) / leaf > 4 (r <= 5, as dense_segment),
+ *   max_slope_deg outside [0, 90), max_curvature NaN or negative, min_size < 1, cap < 0, a NULL params or n_out,
+ *   NULL patches with cap > 0.  LOAM_B200_ERR_STATE without a target.
+ * dense_segment_above_ground: dense_segment's arguments, semantics, records, ranking and errors over the entries that
+ *   are not ground (a voxel of a patch dropped by min_size is an entry); entry indices, first and ties are target
+ *   indices; labels cover the whole target in key order, -1 for a ground voxel.  When no voxel is ground it equals
+ *   dense_segment bit for bit.  LOAM_B200_ERR_STATE without a target or without ground flags.
+ * dense_ground_cloud: per point p of xyzi (n float[4], w ignored; host memory, or device memory when on_device != 0):
+ *   q = pointAssociateToMap(pose, p) as dense_align_iterate computes it (fp32, no FMA); its match is the alignment's
+ *   rule restricted to the ground voxels (the first smallest d2 among the ground voxels of q's search_radius box,
+ *   accepted when d2 < gate, gate = s * s, s = (float)search_radius * leaf); the point is ground when it has a match
+ *   and |pd| <= max_height, pd = (nx*(qx - cx) + ny*(qy - cy)) + nz*(qz - cz) in fp32.
+ *   labels (host, may be NULL): int8 per point, 1 ground, 0 not ground, -1 not finite or q's voxel outside the key
+ *   range.  nonground (may be NULL; host memory when on_device == 0, device memory otherwise, so that it can go
+ *   straight into cloud_segment with on_device = 1): the points labelled 0 in input order, room for n points needed.
+ *   *n_nonground: their number.  LOAM_B200_ERR_ARG: dense_align_iterate's (n < 0, NULL xyzi with n > 0, a NULL or
+ *   non-finite pose, search_radius outside 1..3), max_height not finite or negative, NULL n_nonground.
+ *   LOAM_B200_ERR_STATE without a target or without ground flags.
+ * Every argument check runs on the host before anything is launched, so a refused call changes nothing.  Launches,
+ * with seg(m) = dense_segment's launches for a target of m voxels (0 for m = 0): dense_ground 5 + seg(candidates);
+ * dense_segment_above_ground 4 + seg(entries); dense_ground_cloud 3, plus 1 with nonground; none for an empty target
+ * or cloud.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  float max_slope_deg;  /* the steepest normal tilt from y that is still ground, [0, 90) */
+  float max_curvature;  /* the largest curvature (normal w) that is still ground; +inf: no curvature test */
+  float tol;            /* horizontal joining distance, metres */
+  float max_step;       /* largest height step between joined voxels, metres */
+  int min_size;         /* voxels of the smallest patch kept as ground */
+} loam_b200_ground_params;
+
+int loam_b200_dense_ground(loam_b200_ctx* ctx, const loam_b200_ground_params* params, int32_t* labels,
+                           loam_b200_segment* patches, int cap, int* n_out);
+int loam_b200_dense_segment_above_ground(loam_b200_ctx* ctx, float tol, int min_size, int max_size, int32_t* labels,
+                                         loam_b200_segment* segments, int cap, int* n_out);
+int loam_b200_dense_ground_cloud(loam_b200_ctx* ctx, const float* xyzi, int n, int on_device,
+                                 const loam_b200_pose* pose, int search_radius, float max_height, int8_t* labels,
+                                 float* nonground, int* n_nonground);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU).  With a shard set, loam_b200_map_iterate evaluates this rank's contiguous slice
  * of the corner and surface queries; with a communicator the 32-float partial normal equations are all-reduced
  * (NCCL, sum, fp32) on the context's stream directly behind the kernel, so every rank returns the same totals and

@@ -177,6 +177,18 @@ int loam_b200_map_dense_relocalize_global(void* h, const float* xyzi, int n, int
 int loam_b200_map_dense_target_size(void* h, int* n_out);
 int loam_b200_map_dense_segment(void* h, float tol, int min_size, int max_size, int* labels,
                                 loam_b200_segment* segments, int cap, int* n_out);
+/* Ground of that target (BasicLaserMapping::groundDenseTarget / segmentDenseTargetAboveGround / splitGround,
+ * include/loam_b200.h "Ground of the whole-run voxel map"), same in-flight rule and label / record conventions as
+ * loam_b200_map_dense_segment.  ground_cloud: the points of xyzi (sensor frame, at pose6) labelled ground go to
+ * ground[0 .. *n_ground), those labelled not ground to nonground[0 .. *n_nonground), each in input order (either
+ * array may be NULL; room for n points each). */
+int loam_b200_map_dense_ground(void* h, const loam_b200_ground_params* params, int* labels,
+                               loam_b200_segment* patches, int cap, int* n_out);
+int loam_b200_map_dense_segment_above_ground(void* h, float tol, int min_size, int max_size, int* labels,
+                                             loam_b200_segment* segments, int cap, int* n_out);
+int loam_b200_map_dense_ground_cloud(void* h, const float* xyzi, int n, const float* pose6, int search_radius,
+                                     float max_height, float* ground, int* n_ground, float* nonground,
+                                     int* n_nonground);
 /* multi-GPU, one process per GPU: rank 0 calls loam_b200_host_nccl_unique_id and distributes the 128 bytes; every rank
  * then enables sharding on its mapping object (nccl_id128 = NULL: slice the queries only, no collective) */
 int loam_b200_host_nccl_unique_id(unsigned char* out128);

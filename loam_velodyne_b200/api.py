@@ -115,6 +115,16 @@ class Segment(C.Structure):
                 ("centroid", C.c_float * 3)]
 
 
+class GroundParams(C.Structure):
+    """loam_b200_ground_params; default(): the recommended starting point (DESIGN.md "Ground patches")."""
+    _fields_ = [("max_slope_deg", C.c_float), ("max_curvature", C.c_float), ("tol", C.c_float),
+                ("max_step", C.c_float), ("min_size", C.c_int)]
+
+    @staticmethod
+    def default():
+        return GroundParams(np.float32(15.0), np.float32(0.05), np.float32(0.3), np.float32(0.2), 200)
+
+
 class NormalEq(C.Structure):
     _fields_ = [("AtA", C.c_float * 36), ("AtB", C.c_float * 6), ("n_selected", C.c_int),
                 ("n_corner_selected", C.c_int)]
@@ -259,6 +269,11 @@ def lib():
         "loam_b200_dense_segment": (C.c_int, [vp, C.c_float, C.c_int, C.c_int, _I, C.POINTER(Segment), C.c_int, _I]),
         "loam_b200_cloud_segment": (C.c_int, [vp, _F, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _I,
                                               C.POINTER(Segment), C.c_int, _I]),
+        "loam_b200_dense_ground": (C.c_int, [vp, C.POINTER(GroundParams), _I, C.POINTER(Segment), C.c_int, _I]),
+        "loam_b200_dense_segment_above_ground": (C.c_int, [vp, C.c_float, C.c_int, C.c_int, _I, C.POINTER(Segment),
+                                                           C.c_int, _I]),
+        "loam_b200_dense_ground_cloud": (C.c_int, [vp, _F, C.c_int, C.c_int, C.POINTER(Pose), C.c_int, C.c_float, _B,
+                                                   _F, _I]),
         "loam_b200_comm_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_init": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_comm_destroy": (C.c_int, [vp]),
@@ -332,6 +347,10 @@ def lib():
         "loam_b200_map_dense_target_size": (C.c_int, [vp, _I]),
         "loam_b200_map_dense_segment": (C.c_int, [vp, C.c_float, C.c_int, C.c_int, _I, C.POINTER(Segment), C.c_int,
                                                   _I]),
+        "loam_b200_map_dense_ground": (C.c_int, [vp, C.POINTER(GroundParams), _I, C.POINTER(Segment), C.c_int, _I]),
+        "loam_b200_map_dense_segment_above_ground": (C.c_int, [vp, C.c_float, C.c_int, C.c_int, _I,
+                                                               C.POINTER(Segment), C.c_int, _I]),
+        "loam_b200_map_dense_ground_cloud": (C.c_int, [vp, _F, C.c_int, _F, C.c_int, C.c_float, _F, _I, _F, _I]),
         "loam_b200_host_nccl_unique_id": (C.c_int, [C.POINTER(C.c_ubyte)]),
         "loam_b200_map_enable_sharding": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(C.c_ubyte)]),
         "loam_b200_map_kernel_profile": (C.c_int, [vp, C.c_int, _D]),
@@ -952,6 +971,46 @@ class Ctx:
             self.h, ptr, k, 1 if on_device else 0, np.float32(tolerance), int(min_size), _max_size(max_size), lab,
             seg, cap, kk), k, lambda rc: self._ck(rc, "segment_cloud"))
 
+    # ---- ground (include/loam_b200.h "Ground of the whole-run voxel map"; y is up)
+    def dense_ground(self, params=None):
+        """Ground patches of the target (params: GroundParams, default GroundParams.default()) -> (labels int32[N]:
+        per target voxel in key order, its patch's rank or -1; patches: dict of arrays as dense_segment).  The ground
+        flags stay with the target for dense_segment_above_ground and dense_ground_cloud."""
+        prm = params if params is not None else GroundParams.default()
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_target_size(self.h, C.byref(n)), "dense_ground")
+        return _segment_call(lambda lab, seg, cap, k: self.L.loam_b200_dense_ground(
+            self.h, C.byref(prm), lab, seg, cap, k), n.value, lambda rc: self._ck(rc, "dense_ground"))
+
+    def dense_segment_above_ground(self, tolerance, min_size=1, max_size=None):
+        """dense_segment over the target voxels that are not ground (after dense_ground) -> as dense_segment, labels
+        over the whole target with -1 on the ground."""
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_target_size(self.h, C.byref(n)), "dense_segment_above_ground")
+        return _segment_call(lambda lab, seg, cap, k: self.L.loam_b200_dense_segment_above_ground(
+            self.h, np.float32(tolerance), int(min_size), _max_size(max_size), lab, seg, cap, k), n.value,
+            lambda rc: self._ck(rc, "dense_segment_above_ground"))
+
+    def dense_ground_cloud(self, pts, twist6, search_radius=1, max_height=0.1, on_device=False, n=None, out=None):
+        """Ground points of sensor-frame pts (N x 4) at twist6 against the target's ground -> (labels int8[N]: 1
+        ground, 0 not ground, -1 not finite or outside the key range; the points labelled 0 in input order, K x 4).
+        With on_device=True, pts is the address of n float[4] in device memory and out that of room for n float[4]
+        in device memory (or None): the second value is then K, the points being at out."""
+        ptr, k = _pts_or_device(pts, on_device, n)
+        p = make_pose(twist6)
+        labels = np.zeros(max(k, 1), np.int8)
+        if on_device:
+            dst = None if out is None else C.cast(C.c_void_p(int(out)), _F)
+        else:
+            ng = np.zeros((max(k, 1), 4), np.float32)
+            dst = _fp(ng)
+        kk = C.c_int(0)
+        self._ck(self.L.loam_b200_dense_ground_cloud(self.h, ptr, k, 1 if on_device else 0, C.byref(p),
+                                                     int(search_radius), np.float32(max_height),
+                                                     labels.ctypes.data_as(_B), dst, C.byref(kk)),
+                 "dense_ground_cloud")
+        return labels[:k].copy(), (kk.value if on_device else ng[:kk.value].copy())
+
     # ---- place recognition (include/loam_b200.h "Place recognition and global relocalisation")
     def place_descriptor(self, pts, params=None, on_device=False, n=None):
         """Polar height descriptor of sensor-frame pts (N x 4, w ignored) -> float32 (rings, sectors).  With
@@ -1460,6 +1519,36 @@ class LaserMapping(_Handle):
         return _segment_call(lambda lab, seg, cap, k: self.L.loam_b200_map_dense_segment(
             self.h, np.float32(tolerance), int(min_size), _max_size(max_size), lab, seg, cap, k), n.value,
             lambda rc: self._ck(rc, "segmentDenseTarget"))
+
+    def ground_dense_target(self, params=None):
+        """BasicLaserMapping::groundDenseTarget; returns what Ctx.dense_ground returns."""
+        prm = params if params is not None else GroundParams.default()
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_map_dense_target_size(self.h, C.byref(n)), "groundDenseTarget")
+        return _segment_call(lambda lab, seg, cap, k: self.L.loam_b200_map_dense_ground(
+            self.h, C.byref(prm), lab, seg, cap, k), n.value, lambda rc: self._ck(rc, "groundDenseTarget"))
+
+    def segment_dense_target_above_ground(self, tolerance, min_size=1, max_size=None):
+        """BasicLaserMapping::segmentDenseTargetAboveGround; returns what Ctx.dense_segment_above_ground returns."""
+        n = C.c_int(0)
+        self._ck(self.L.loam_b200_map_dense_target_size(self.h, C.byref(n)), "segmentDenseTargetAboveGround")
+        return _segment_call(lambda lab, seg, cap, k: self.L.loam_b200_map_dense_segment_above_ground(
+            self.h, np.float32(tolerance), int(min_size), _max_size(max_size), lab, seg, cap, k), n.value,
+            lambda rc: self._ck(rc, "segmentDenseTargetAboveGround"))
+
+    def split_ground(self, pts, twist6, search_radius=1, max_height=0.1):
+        """BasicLaserMapping::splitGround -> (ground points, other finite points), each K x 4 in input order: the
+        points Ctx.dense_ground_cloud labels 1 and 0."""
+        a = _pts(pts)
+        t = np.ascontiguousarray(twist6, np.float32).reshape(6)
+        k = a.shape[0]
+        g = np.zeros((max(k, 1), 4), np.float32)
+        ng = np.zeros((max(k, 1), 4), np.float32)
+        kg, kn = C.c_int(0), C.c_int(0)
+        self._ck(self.L.loam_b200_map_dense_ground_cloud(self.h, _fp(a), k, _fp(t), int(search_radius),
+                                                         np.float32(max_height), _fp(g), C.byref(kg), _fp(ng),
+                                                         C.byref(kn)), "splitGround")
+        return g[:kg.value].copy(), ng[:kn.value].copy()
 
     def build_dense_distance_field(self, lo, dims, max_distance, download=True):
         """BasicLaserMapping::buildDenseDistanceField; as Ctx.dense_distance_field."""

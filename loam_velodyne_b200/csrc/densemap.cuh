@@ -563,6 +563,28 @@ __global__ void dense_target_gather_kernel(const unsigned long long* __restrict_
   else if (i > 0 && keys64[order[i - 1]] == k) atomicOr(bad, 2);
 }
 
+// The alignment's match of a map-frame point q whose voxel is `key`: among the target voxels of dense_box_walk that
+// use(j) admits, the first smallest d2 = (dx*dx + dy*dy) + dz*dz, d = c - q in fp32, below the gate (strict <); -1
+// when none.  dense_align_kernel admits the voxels with a normal, dense_ground_cloud_kernel the ground voxels.
+template <typename F>
+__device__ __forceinline__ int dense_match(const unsigned long long* __restrict__ skey, const float4* __restrict__ cent,
+                                           int m, unsigned long long key, int radius, float gate, float qx, float qy,
+                                           float qz, F&& use) {
+  int best = -1;
+  float best_d2 = gate;  // strict < from the gate: the first smallest d2 below it
+  dense_box_walk(skey, m, key, radius, [&](int j) {
+    if (!use(j)) return;
+    const float4 c = cent[j];
+    const float dx = c.x - qx, dy = c.y - qy, dz = c.z - qz;
+    const float d2 = (dx * dx + dy * dy) + dz * dz;
+    if (d2 < best_d2) {
+      best_d2 = d2;
+      best = j;
+    }
+  });
+  return best;
+}
+
 // One Gauss-Newton iteration of a cloud against the target, one thread per point (point i in CTA i / LM_THREADS):
 //   q = associate_to_map(pose, p); v = voxel of q (dense_key_of with the target's leaf);
 //   candidates: the target voxels of dense_box_walk around v whose normal_x is not NaN; the first smallest d2 = (dx*dx + dy*dy) + dz*dz, d = c - q, wins when d2 < gate;
@@ -662,19 +684,8 @@ dense_align_kernel(const unsigned long long* __restrict__ skey, const float4* __
       float qx, qy, qz;
       associate_to_map(a, po, qx, qy, qz);
       const unsigned long long key = dense_key_of(make_float4(qx, qy, qz, 0.f), inv);
-      if (key != DENSE_EMPTY) {
-        float best_d2 = gate;  // strict < from the gate: the first smallest d2 below it
-        dense_box_walk(skey, m, key, radius, [&](int j) {
-          if (isnan(nrm[j].x)) return;
-          const float4 c = cent[j];
-          const float dx = c.x - qx, dy = c.y - qy, dz = c.z - qz;
-          const float d2 = (dx * dx + dy * dy) + dz * dz;
-          if (d2 < best_d2) {
-            best_d2 = d2;
-            best = j;
-          }
-        });
-      }
+      if (key != DENSE_EMPTY)
+        best = dense_match(skey, cent, m, key, radius, gate, qx, qy, qz, [&](int j) { return !isnan(nrm[j].x); });
       if (best >= 0) {
         const float4 c = cent[best], nv = nrm[best];
         const float pd2 = (nv.x * (qx - c.x) + nv.y * (qy - c.y)) + nv.z * (qz - c.z);
@@ -1719,6 +1730,99 @@ __global__ void dense_seg_record_kernel(const int* __restrict__ kept, const int*
   out[r] = g;
 }
 
+// ---- ground patches (include/loam_b200.h "Ground of the whole-run voxel map")
+// The candidates and the above-ground entries are the target voxels of class 0, compacted in key order by
+// compact_count_kernel<0> at limit 1 and radix_scan_kernel; the compaction of sorted keys is sorted, so dense_box_walk
+// and the dense_seg_* kernels run on it unchanged, and the entry order (compacted position) is the target order.
+
+// class per target voxel: 0 a candidate (normal_x not NaN, (double)|n_y| >= cos_max, n_w <= max_curv unless
+// check_curv is 0; a NaN w fails), 1 not
+__global__ void dense_ground_candidate_kernel(const float4* __restrict__ nrm, int n, double cos_max, float max_curv,
+                                              int check_curv, unsigned char* __restrict__ cls) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 v = nrm[i];
+  const bool cand = !isnan(v.x) && (double)fabsf(v.y) >= cos_max && (!check_curv || v.w <= max_curv);
+  cls[i] = cand ? 0 : 1;
+}
+
+// the selected target voxels at their compacted position: key, centroid, target index
+__global__ void dense_ground_compact_kernel(const unsigned long long* __restrict__ skey,
+                                            const float4* __restrict__ cent, int n,
+                                            const unsigned* __restrict__ local_pos,
+                                            const unsigned* __restrict__ block_off, unsigned long long* __restrict__ ckey,
+                                            float4* __restrict__ cpos, int* __restrict__ orig) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned pv = local_pos[i];
+  if (!(pv >> 31)) return;
+  const unsigned d = (pv & 0x7fffffffu) + block_off[i / SCAN_BS];
+  ckey[d] = skey[i];
+  cpos[d] = cent[i];
+  orig[d] = i;
+}
+
+// dense_seg_union_kernel with the ground edge: horizontal d2 = dx*dx + dz*dz <= tol2 and |dy| <= max_step, fp64 of
+// the float centroids without FMA (y is up)
+__global__ void __launch_bounds__(128)
+dense_ground_union_kernel(const unsigned long long* __restrict__ skey, const float4* __restrict__ spos, int n,
+                          int radius, double tol2, double max_step, int* par) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 pi = spos[i];
+  const double px = (double)pi.x, py = (double)pi.y, pz = (double)pi.z;
+  dense_box_walk(skey, n, skey[i], radius, [&](int j) {
+    if (j <= i) return;
+    const float4 pj = spos[j];
+    const double dx = px - (double)pj.x, dy = py - (double)pj.y, dz = pz - (double)pj.z;
+    if (dx * dx + dz * dz <= tol2 && fabs(dy) <= max_step) dense_seg_unite(par, i, j);
+  });
+}
+
+// one thread per target voxel e: its label from the compacted labels clab (-1 when it was not selected), with
+// `ground` its ground flag (label >= 0); the first *kept records' `first` from compacted position to target index
+__global__ void dense_ground_scatter_kernel(int n, const unsigned* __restrict__ local_pos,
+                                            const unsigned* __restrict__ block_off, const int* __restrict__ clab,
+                                            const int* __restrict__ orig, const int* __restrict__ kept,
+                                            loam_b200_segment* __restrict__ seg, int* __restrict__ labels,
+                                            unsigned char* __restrict__ ground) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const unsigned pv = local_pos[e];
+  const int lab = (pv >> 31) ? clab[(pv & 0x7fffffffu) + block_off[e / SCAN_BS]] : -1;
+  labels[e] = lab;
+  if (ground) ground[e] = lab >= 0 ? 1 : 0;
+  if (kept && e < *kept) seg[e].first = orig[seg[e].first];
+}
+
+// One thread per point: q = associate_to_map(pose, p) and dense_match over the ground voxels; class 1 ground (a match
+// with |pd| <= max_height, pd = (nx*(qx - cx) + ny*(qy - cy)) + nz*(qz - cz) in fp32), 0 not ground, 0xff (-1) for
+// a point that is not finite or whose voxel lies outside the key range
+__global__ void dense_ground_cloud_kernel(const unsigned long long* __restrict__ skey, const float4* __restrict__ cent,
+                                          const float4* __restrict__ nrm, const unsigned char* __restrict__ ground,
+                                          int m, float inv, int radius, float gate, const float4* __restrict__ pts,
+                                          int n, MapIterArgs a, float max_height, unsigned char* __restrict__ cls) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 po = pts[i];
+  unsigned char l = 0xff;
+  if (isfinite(po.x) && isfinite(po.y) && isfinite(po.z)) {
+    float qx, qy, qz;
+    associate_to_map(a, po, qx, qy, qz);
+    const unsigned long long key = dense_key_of(make_float4(qx, qy, qz, 0.f), inv);
+    if (key != DENSE_EMPTY) {
+      const int best = dense_match(skey, cent, m, key, radius, gate, qx, qy, qz, [&](int j) { return ground[j] != 0; });
+      l = 0;
+      if (best >= 0) {
+        const float4 c = cent[best], nv = nrm[best];
+        const float pd = (nv.x * (qx - c.x) + nv.y * (qy - c.y)) + nv.z * (qz - c.z);
+        if (fabsf(pd) <= max_height) l = 1;
+      }
+    }
+  }
+  cls[i] = l;
+}
+
 // Scratch of one segmentation: DenseTarget::seg for the target, loam_b200_ctx::seg for clouds; kept for the next call
 struct DenseSegScratch {
   DevBuf<unsigned long long> keys64, skey;  // cloud: input keys, sorted keys
@@ -1851,7 +1955,14 @@ struct DenseTarget {
   DevBuf<float> dist_f;                 // the float distances of a build that downloads them
   DevBuf<int> edt_g, edt_b, edt_s, edt_t, edt_v;
   DevBuf<float> qdist, qgrad;
-  DenseSegScratch seg;                  // loam_b200_dense_segment
+  DenseSegScratch seg;                  // loam_b200_dense_segment (and the ground calls' compacted entries)
+  // ground of loam_b200_dense_ground: one flag per voxel in key order (ground_ready false: none; a build, load or
+  // release drops it, the next dense_ground replaces it); the scratch of the ground calls
+  bool ground_ready = false;
+  DevBuf<unsigned char> ground, gcls;   // flags; classes of the compaction (target voxels, or a cloud's points)
+  DevBuf<unsigned> gpos, gbsum;         // compact_count_kernel's local positions and block sums
+  DevBuf<int> glabels;                  // labels in target order
+  DevBuf<float4> gout;                  // ground_cloud: the points that are not ground, for a host copy
 
   void release() {
     keys.release(); keys64.release(); cent.release(); nrm.release(); pts.release(); args.release(); partials.release();
@@ -1865,6 +1976,8 @@ struct DenseTarget {
     dist_sq.release(); dist_f.release(); edt_g.release(); edt_b.release(); edt_s.release(); edt_t.release();
     edt_v.release(); qdist.release(); qgrad.release();
     seg.release();
+    ground.release(); gcls.release(); gpos.release(); gbsum.release(); glabels.release(); gout.release();
+    ground_ready = false;
     dist_ready = false;
     ray = DenseBrickIndex{};
     n = 0;

@@ -204,21 +204,18 @@ size_t BasicLaserMapping::denseTargetSize() {
   return (size_t)n;
 }
 
-std::vector<BasicLaserMapping::DenseSegment> BasicLaserMapping::segmentDenseTarget(float tolerance, int minSize,
-                                                                                   int maxSize,
-                                                                                   std::vector<int>* labels) {
-  const size_t n = denseTargetSize();  // the labels' length, and K <= n
+// One segmentation of the target through the C ABI: call(labels or nullptr, records, cap, &k) with room for the n
+// target voxels' labels and n records (K <= n), the records converted
+template <typename F>
+static std::vector<BasicLaserMapping::DenseSegment> targetSegments(size_t n, std::vector<int>* labels, F&& call) {
   std::vector<loam_b200_segment> seg(n + 1);
   std::vector<int32_t> lab(labels ? n + 1 : 0);
-  int k = 0;
-  _gpu->check(loam_b200_dense_segment(_gpu->get(), tolerance, minSize, maxSize, labels ? lab.data() : nullptr,
-                                      seg.data(), (int)n, &k),
-              "loam_b200_dense_segment");
+  const int k = call(labels ? lab.data() : nullptr, seg.data(), (int)n);
   if (labels) labels->assign(lab.begin(), lab.begin() + (ptrdiff_t)n);
-  std::vector<DenseSegment> out((size_t)k);
+  std::vector<BasicLaserMapping::DenseSegment> out((size_t)k);
   for (int i = 0; i < k; i++) {
     const loam_b200_segment& g = seg[(size_t)i];
-    DenseSegment& o = out[(size_t)i];
+    BasicLaserMapping::DenseSegment& o = out[(size_t)i];
     o.size = (size_t)g.size;
     o.first = (size_t)g.first;
     for (int a = 0; a < 3; a++) {
@@ -228,6 +225,58 @@ std::vector<BasicLaserMapping::DenseSegment> BasicLaserMapping::segmentDenseTarg
     }
   }
   return out;
+}
+
+std::vector<BasicLaserMapping::DenseSegment> BasicLaserMapping::segmentDenseTarget(float tolerance, int minSize,
+                                                                                   int maxSize,
+                                                                                   std::vector<int>* labels) {
+  return targetSegments(denseTargetSize(), labels, [&](int32_t* lab, loam_b200_segment* seg, int cap) {
+    int k = 0;
+    _gpu->check(loam_b200_dense_segment(_gpu->get(), tolerance, minSize, maxSize, lab, seg, cap, &k),
+                "loam_b200_dense_segment");
+    return k;
+  });
+}
+
+std::vector<BasicLaserMapping::DenseSegment> BasicLaserMapping::groundDenseTarget(const DenseGroundParams& params,
+                                                                                  std::vector<int>* labels) {
+  const loam_b200_ground_params prm{params.maxSlopeDeg, params.maxCurvature, params.tolerance, params.maxStep,
+                                    params.minSize};
+  return targetSegments(denseTargetSize(), labels, [&](int32_t* lab, loam_b200_segment* seg, int cap) {
+    int k = 0;
+    _gpu->check(loam_b200_dense_ground(_gpu->get(), &prm, lab, seg, cap, &k), "loam_b200_dense_ground");
+    return k;
+  });
+}
+
+std::vector<BasicLaserMapping::DenseSegment> BasicLaserMapping::segmentDenseTargetAboveGround(float tolerance,
+                                                                                              int minSize, int maxSize,
+                                                                                              std::vector<int>* labels) {
+  return targetSegments(denseTargetSize(), labels, [&](int32_t* lab, loam_b200_segment* seg, int cap) {
+    int k = 0;
+    _gpu->check(loam_b200_dense_segment_above_ground(_gpu->get(), tolerance, minSize, maxSize, lab, seg, cap, &k),
+                "loam_b200_dense_segment_above_ground");
+    return k;
+  });
+}
+
+void BasicLaserMapping::splitGround(const Cloud& cloud, const Twist& pose, Cloud& ground, Cloud& nonGround,
+                                    int searchRadius, float maxHeight) {
+  b200::pack(cloud, _bufA);
+  loam_b200_pose p;
+  b200::fillPose(pose, p);
+  const size_t n = cloud.points.size();
+  std::vector<int8_t> lab(n + 1);
+  int k = 0;
+  _gpu->check(loam_b200_dense_ground_cloud(_gpu->get(), _bufA.data(), (int)n, 0, &p, searchRadius, maxHeight,
+                                           lab.data(), nullptr, &k),
+              "loam_b200_dense_ground_cloud");
+  ground.clear();
+  nonGround.clear();
+  for (size_t i = 0; i < n; i++) {
+    if (lab[i] == 1) ground.push_back(cloud.points[i]);
+    else if (lab[i] == 0) nonGround.push_back(cloud.points[i]);
+  }
 }
 
 static Twist twistOf(const float rot[3], const float pos[3]) {

@@ -797,6 +797,26 @@ int loam_b200_map_dense_target_size(void* h, int* n_out) {
     return 0;
   });
 }
+// the records and labels of a target segmentation by the drop-in class: ERR_CAPACITY when they exceed cap
+static int put_segments(const char* what, const std::vector<loam::BasicLaserMapping::DenseSegment>& seg,
+                        const std::vector<int>& lab, int* labels, loam_b200_segment* segments, int cap, int* n_out) {
+  *n_out = (int)seg.size();
+  if ((int)seg.size() > cap) {
+    g_err = std::string(what) + ": output capacity too small";
+    return (int)LOAM_B200_ERR_CAPACITY;
+  }
+  for (size_t i = 0; i < seg.size(); i++) {
+    segments[i].size = (int32_t)seg[i].size;
+    segments[i].first = (int32_t)seg[i].first;
+    for (int a = 0; a < 3; a++) {
+      segments[i].lo[a] = seg[i].lo[a];
+      segments[i].hi[a] = seg[i].hi[a];
+      segments[i].centroid[a] = seg[i].centroid[a];
+    }
+  }
+  if (labels && !lab.empty()) std::memcpy(labels, lab.data(), lab.size() * sizeof(int));
+  return 0;
+}
 int loam_b200_map_dense_segment(void* h, float tol, int min_size, int max_size, int* labels,
                                 loam_b200_segment* segments, int cap, int* n_out) {
   if (const int rc = map_in_flight((MapH*)h)) return rc;
@@ -808,21 +828,60 @@ int loam_b200_map_dense_segment(void* h, float tol, int min_size, int max_size, 
     auto* m = (MapH*)h;
     std::vector<int> lab;
     const auto seg = m->m.segmentDenseTarget(tol, min_size, max_size, labels ? &lab : nullptr);
-    *n_out = (int)seg.size();
-    if ((int)seg.size() > cap) {
-      g_err = "loam_b200_map_dense_segment: output capacity too small";
-      return (int)LOAM_B200_ERR_CAPACITY;
-    }
-    for (size_t i = 0; i < seg.size(); i++) {
-      segments[i].size = (int32_t)seg[i].size;
-      segments[i].first = (int32_t)seg[i].first;
-      for (int a = 0; a < 3; a++) {
-        segments[i].lo[a] = seg[i].lo[a];
-        segments[i].hi[a] = seg[i].hi[a];
-        segments[i].centroid[a] = seg[i].centroid[a];
-      }
-    }
-    if (labels && !lab.empty()) std::memcpy(labels, lab.data(), lab.size() * sizeof(int));
+    return put_segments("loam_b200_map_dense_segment", seg, lab, labels, segments, cap, n_out);
+  });
+}
+int loam_b200_map_dense_ground(void* h, const loam_b200_ground_params* params, int* labels,
+                               loam_b200_segment* patches, int cap, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (!params || cap < 0 || (cap > 0 && !patches) || !n_out) {
+    g_err = "loam_b200_map_dense_ground: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    loam::BasicLaserMapping::DenseGroundParams prm;
+    prm.maxSlopeDeg = params->max_slope_deg;
+    prm.maxCurvature = params->max_curvature;
+    prm.tolerance = params->tol;
+    prm.maxStep = params->max_step;
+    prm.minSize = params->min_size;
+    std::vector<int> lab;
+    const auto seg = m->m.groundDenseTarget(prm, labels ? &lab : nullptr);
+    return put_segments("loam_b200_map_dense_ground", seg, lab, labels, patches, cap, n_out);
+  });
+}
+int loam_b200_map_dense_segment_above_ground(void* h, float tol, int min_size, int max_size, int* labels,
+                                             loam_b200_segment* segments, int cap, int* n_out) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (cap < 0 || (cap > 0 && !segments) || !n_out) {
+    g_err = "loam_b200_map_dense_segment_above_ground: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    std::vector<int> lab;
+    const auto seg = m->m.segmentDenseTargetAboveGround(tol, min_size, max_size, labels ? &lab : nullptr);
+    return put_segments("loam_b200_map_dense_segment_above_ground", seg, lab, labels, segments, cap, n_out);
+  });
+}
+int loam_b200_map_dense_ground_cloud(void* h, const float* xyzi, int n, const float* pose6, int search_radius,
+                                     float max_height, float* ground, int* n_ground, float* nonground,
+                                     int* n_nonground) {
+  if (const int rc = map_in_flight((MapH*)h)) return rc;
+  if (n < 0 || (n > 0 && !xyzi) || !pose6 || !n_ground || !n_nonground) {
+    g_err = "loam_b200_map_dense_ground_cloud: bad size or NULL argument";
+    return (int)LOAM_B200_ERR_ARG;
+  }
+  return guarded([&] {
+    auto* m = (MapH*)h;
+    fill(m->scratchA, xyzi, n);
+    Cloud g, ng;
+    m->m.splitGround(m->scratchA, twists_of(pose6, 1)[0], g, ng, search_radius, max_height);
+    *n_ground = (int)g.points.size();
+    *n_nonground = (int)ng.points.size();
+    if (ground) dump(g, ground);
+    if (nonground) dump(ng, nonground);
     return 0;
   });
 }

@@ -288,6 +288,28 @@ class BasicLaserMapping {
   size_t denseTargetSize();
   std::vector<DenseSegment> segmentDenseTarget(float tolerance, int minSize = 1, int maxSize = 2147483647,
                                                std::vector<int>* labels = nullptr);
+  // Ground of the target (include/loam_b200.h "Ground of the whole-run voxel map"; y is up).  groundDenseTarget:
+  // patches of voxels whose normal lies within maxSlopeDeg of y and whose curvature is at most maxCurvature (+inf: no
+  // curvature test), joined within `tolerance` metres horizontally and `maxStep` metres vertically, kept from minSize
+  // voxels; ranked and recorded as segmentDenseTarget.  The ground flags stay with the target (until its next build
+  // or load) for the two calls below.  A flat roof with no step to the street is a patch too: reject it by lo[1].
+  // segmentDenseTargetAboveGround: segmentDenseTarget over the voxels that are not ground (labels -1 on the ground).
+  // splitGround: the points of a sensor-frame cloud at `pose` that lie within maxHeight of a ground voxel's plane
+  // (its nearest ground centroid within searchRadius voxels) go to `ground`, the other finite points to `nonGround`,
+  // both in input order.  All throw without a target or ground and on bad arguments.
+  struct DenseGroundParams {
+    DenseGroundParams() : maxSlopeDeg(15.f), maxCurvature(0.05f), tolerance(0.3f), maxStep(0.2f), minSize(200) {}
+    float maxSlopeDeg, maxCurvature;  // degrees from y; the normal's w (+inf: no curvature test)
+    float tolerance, maxStep;         // metres: horizontal joining distance, largest height step
+    int minSize;                      // voxels of the smallest patch
+  };
+  std::vector<DenseSegment> groundDenseTarget(const DenseGroundParams& params = DenseGroundParams(),
+                                              std::vector<int>* labels = nullptr);
+  std::vector<DenseSegment> segmentDenseTargetAboveGround(float tolerance, int minSize = 1,
+                                                          int maxSize = 2147483647, std::vector<int>* labels = nullptr);
+  void splitGround(const pcl::PointCloud<pcl::PointXYZI>& cloud, const Twist& pose,
+                   pcl::PointCloud<pcl::PointXYZI>& ground, pcl::PointCloud<pcl::PointXYZI>& nonGround,
+                   int searchRadius = 1, float maxHeight = 0.1f);
 
  private:
   typedef pcl::PointCloud<pcl::PointXYZI> Cloud;
